@@ -199,6 +199,15 @@ NVC_API const char* nvc_version(void);
  * afterwards (call again after re-uploading; meshes = NULL releases the view). */
 NVC_API int nvc_prepare_meshes(NvcContext* ctx, void* stream, const NvcMesh* meshes, uint32_t mesh_count);
 
+/* Optional, once per geometry upload (where the reference uploads `mlb`, niagara.cpp:1055, next to nvc_prepare_meshes):
+ * builds a context-owned, read-only cull view of Meshlet[] — exact copies of the 12 bytes the cluster tests read, as two dense
+ * arrays: bytes 0-7 of every record (center[3], radius) and bytes 8-11 (cone_axis[3], cone_cutoff).  nvc_clustercull and
+ * nvc_taskcull calls that pass the same `meshlets` pointer then read 12 bytes per meshlet as two coalesced streams instead of
+ * the 24-byte records; any other pointer reads the records.  Results are identical.  The Meshlet[] contents must not change
+ * afterwards (call again after re-uploading; meshlets = NULL releases the view).  Allocates / frees: call outside stream
+ * capture. */
+NVC_API int nvc_prepare_meshlets(NvcContext* ctx, void* stream, const NvcMeshlet* meshlets, uint32_t meshlet_count);
+
 /* Tuning: stage the coarse tail of the depth pyramid (top mips, at most `texels` texels, capped at 11264 = 44 KB) into
  * shared memory once per CTA of the late cluster pass with one TMA bulk copy (cp.async.bulk, SASS UBLKCP); lookups
  * whose whole warp samples a staged mip then read shared memory.  0 (default) disables it: on the measured workloads

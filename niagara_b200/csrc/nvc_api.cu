@@ -238,6 +238,10 @@ NVC_API void nvc_destroy(NvcContext* ctx)
 		cudaFree(ctx->mesh_heads);
 	if (ctx->mesh_errors)
 		cudaFree(ctx->mesh_errors);
+	if (ctx->meshlet_sphere)
+		cudaFree(ctx->meshlet_sphere);
+	if (ctx->meshlet_cone)
+		cudaFree(ctx->meshlet_cone);
 	if (ctx->hiz_fp)
 		cudaFree(ctx->hiz_fp);
 	delete ctx;
@@ -275,6 +279,39 @@ NVC_API int nvc_prepare_meshes(NvcContext* ctx, void* stream, const NvcMesh* mes
 	}
 	ctx->prepared_meshes = meshes;
 	ctx->prepared_mesh_count = mesh_count;
+	return NVC_OK;
+}
+
+NVC_API int nvc_prepare_meshlets(NvcContext* ctx, void* stream, const NvcMeshlet* meshlets, uint32_t meshlet_count)
+{
+	if (!ctx)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	DeviceGuard guard(ctx->device);
+	if (ctx->meshlet_sphere)
+	{
+		cudaDeviceSynchronize();
+		cudaFree(ctx->meshlet_sphere);
+		cudaFree(ctx->meshlet_cone);
+		ctx->meshlet_sphere = nullptr;
+		ctx->meshlet_cone = nullptr;
+		ctx->prepared_meshlets = nullptr;
+	}
+	if (!meshlets || meshlet_count == 0)
+		return NVC_OK; // un-prepare
+	cudaError_t e = cudaMalloc(&ctx->meshlet_sphere, size_t(meshlet_count) * sizeof(uint2));
+	if (e == cudaSuccess)
+		e = cudaMalloc(&ctx->meshlet_cone, size_t(meshlet_count) * sizeof(uint32_t));
+	if (e == cudaSuccess)
+		e = nvc::launch_pack_meshlets(meshlets, meshlet_count, ctx->meshlet_sphere, ctx->meshlet_cone, static_cast<cudaStream_t>(stream));
+	if (e != cudaSuccess)
+	{
+		cudaFree(ctx->meshlet_sphere);
+		cudaFree(ctx->meshlet_cone);
+		ctx->meshlet_sphere = nullptr;
+		ctx->meshlet_cone = nullptr;
+		return e == cudaErrorMemoryAllocation ? NVC_ERROR_OUT_OF_MEMORY : cuda_fail(ctx, e, "nvc_prepare_meshlets");
+	}
+	ctx->prepared_meshlets = meshlets;
 	return NVC_OK;
 }
 
@@ -381,6 +418,19 @@ static int fill_cluster_params(NvcContext* ctx, const NvcCullData* cull, int lat
 	p.command_count4 = command_count4;
 	p.draws = draws;
 	p.meshlets = meshlets;
+	if (ctx->meshlet_sphere && ctx->prepared_meshlets == meshlets)
+	{
+		p.ml_sphere = reinterpret_cast<const char*>(ctx->meshlet_sphere);
+		p.ml_cone = reinterpret_cast<const char*>(ctx->meshlet_cone);
+		p.ml_sphere_stride = sizeof(uint2);
+		p.ml_cone_stride = sizeof(uint32_t);
+	}
+	else
+	{
+		p.ml_sphere = reinterpret_cast<const char*>(meshlets);
+		p.ml_cone = reinterpret_cast<const char*>(meshlets) + 8;
+		p.ml_sphere_stride = p.ml_cone_stride = sizeof(NvcMeshlet);
+	}
 	p.meshlet_visibility = meshlet_visibility;
 	p.scratch = ctx->scratch;
 	p.cluster_limit = ctx->limits.cluster_limit;

@@ -32,6 +32,10 @@ struct NvcContext
 	uint32_t prepared_mesh_count = 0;
 	void* mesh_heads = nullptr;
 	float* mesh_errors = nullptr;
+	// derived meshlet cull view (nvc_prepare_meshlets): bytes 0-7 and 8-11 of every Meshlet record
+	const void* prepared_meshlets = nullptr;
+	uint2* meshlet_sphere = nullptr;
+	uint32_t* meshlet_cone = nullptr;
 	int nccl_rank = 0, nccl_world = 1;
 	// footprint image of one pyramid (nvc_prepare_hiz): keyed by the pyramid's texel pointer and shape
 	float* hiz_fp = nullptr;
@@ -158,6 +162,13 @@ struct ClusterParams
 	const uint32_t* command_count4;
 	const NvcMeshDraw* draws;
 	const NvcMeshlet* meshlets;
+	// Where the 12 bytes the cluster tests read live for meshlet i: bytes 0-7 (center[3], radius as binary16) at
+	// ml_sphere + i * ml_sphere_stride, bytes 8-11 (cone_axis[3], cone_cutoff as s8) at ml_cone + i * ml_cone_stride.
+	// Either the prepared view of `meshlets` (nvc_prepare_meshlets: strides 8 and 4) or the records themselves (stride 24),
+	// resolved on the host so that the kernels' address arithmetic has no branch.
+	const char* ml_sphere;
+	const char* ml_cone;
+	uint32_t ml_sphere_stride, ml_cone_stride;
 	uint32_t* meshlet_visibility;
 	uint32_t* cluster_indices;
 	uint32_t* cluster_count4;
@@ -192,6 +203,7 @@ cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pa
 cudaError_t launch_cook_meshlet_bounds(const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* meshletdata, uint32_t meshletdata_words, NvcMeshlet* meshlets, uint32_t meshlet_count, uint32_t* rejected, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);
+cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream);
 cudaError_t clustercull_occupancy(int* blocks_per_sm_early, int* blocks_per_sm_late, int* blocks_per_sm_late_staged, uint32_t stage_bytes);
 cudaError_t clustercull_filter_occupancy(int* blocks_per_sm_early, int* blocks_per_sm_late);
 uint32_t hiz_stage_bytes(const HiZDesc& hiz);

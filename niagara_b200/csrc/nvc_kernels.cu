@@ -649,14 +649,34 @@ struct ItemData
 	bool have_geom; // d0/d1/b0/b1 were loaded
 };
 
+// The 12 bytes of meshlet `mi` that every cluster test reads: b0 = center[3], radius (4 x binary16), b1 = cone_axis[3],
+// cone_cutoff (4 x s8).  From the prepared view (nvc_prepare_meshlets: 8 + 4 bytes at dense strides, so a warp's loads are
+// fully coalesced) when the pass reads the prepared Meshlet[], else from the first 12 bytes of the 24-byte record: the host
+// sets the bases and strides (ClusterParams), the same two multiply-adds serve both.  STREAM: L2 evict-first loads (policy
+// `pol`), else plain read-only loads.
+template <bool STREAM>
+__device__ __forceinline__ void load_meshlet_cull(const ClusterParams& p, uint32_t mi, uint64_t pol, uint2& b0, uint32_t& b1)
+{
+	const char* sp = p.ml_sphere + size_t(mi) * p.ml_sphere_stride;
+	const char* cp = p.ml_cone + size_t(mi) * p.ml_cone_stride;
+	if (STREAM)
+	{
+		b0 = ldg_stream_u2(sp, pol);
+		b1 = ldg_stream_u32(cp, pol);
+	}
+	else
+	{
+		b0 = __ldg(reinterpret_cast<const uint2*>(sp));
+		b1 = __ldg(reinterpret_cast<const uint32_t*>(cp));
+	}
+}
+
 __device__ __forceinline__ void load_geometry(const ClusterParams& p, const ItemRef& r, ItemData& d)
 {
 	const char* dp = reinterpret_cast<const char*>(p.draws + r.drawId);
 	d.d0 = ldg_f4(dp);
 	d.d1 = ldg_f4(dp + 16);
-	const char* mp = reinterpret_cast<const char*>(p.meshlets + r.mi);
-	d.b0 = __ldg(reinterpret_cast<const uint2*>(mp));
-	d.b1 = __ldg(reinterpret_cast<const uint32_t*>(mp + 8));
+	load_meshlet_cull<false>(p, r.mi, 0, d.b0, d.b1);
 }
 
 // Issues the loads of one chunk.  LATE: everything an active lane needs (bit word + geometry).  EARLY: only the bit
@@ -1373,14 +1393,11 @@ __global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : 
 				b0 = make_uint2(0u, 0u);
 				b1 = 0u;
 				if (active)
-				{
-					const char* mp = reinterpret_cast<const char*>(p.meshlets + (ids.x + mgi));
-					b0 = ldg_stream_u2(mp, spol);
-					b1 = ldg_stream_u32(mp + 8, spol);
-				}
+					load_meshlet_cull<true>(p, ids.x + mgi, spol, b0, b1);
 			};
 
-			// NVC_FILTER_PIPELINE = prefetch distance in chunks (0: none).  Distance 2 keeps two chunks (2 x 768 bytes per warp) in
+			// NVC_FILTER_PIPELINE = prefetch distance in chunks (0: none).  Distance 2 keeps two chunks (2 x 384 bytes per warp from
+			// the meshlet cull view, 2 x 768 from the 24-byte records) in
 			// flight: with one, a chunk's arithmetic (~0.6 us at 8 warps per scheduler) is shorter than the DRAM latency under load
 			uint32_t n_jm = 0, n_b1 = 0, m_jm = 0, m_b1 = 0;
 			uint2 n_b0 = make_uint2(0u, 0u), m_b0 = make_uint2(0u, 0u);
@@ -2224,6 +2241,25 @@ cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHe
 	if (count == 0)
 		return cudaSuccess;
 	pack_meshes_kernel<<<(count + 255) / 256, 256, 0, stream>>>(meshes, count, heads, errors);
+	return cudaGetLastError();
+}
+
+// the meshlet cull view (nvc_prepare_meshlets): bytes 0-7 and 8-11 of every 24-byte record, copied unchanged
+__global__ void pack_meshlets_kernel(const NvcMeshlet* __restrict__ meshlets, uint32_t count, uint2* __restrict__ sphere, uint32_t* __restrict__ cone)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= count)
+		return;
+	const char* mp = reinterpret_cast<const char*>(meshlets + i);
+	sphere[i] = *reinterpret_cast<const uint2*>(mp);
+	cone[i] = *reinterpret_cast<const uint32_t*>(mp + 8);
+}
+
+cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream)
+{
+	if (count == 0)
+		return cudaSuccess;
+	pack_meshlets_kernel<<<(count + 255) / 256, 256, 0, stream>>>(meshlets, count, sphere, cone);
 	return cudaGetLastError();
 }
 

@@ -26,6 +26,7 @@ SIGNATURES = [
     ("nvc_last_error", ctypes.c_char_p, [c_void_p]),
     ("nvc_version", ctypes.c_char_p, []),
     ("nvc_prepare_meshes", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_uint32]),
+    ("nvc_prepare_meshlets", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_uint32]),
     ("nvc_set_hiz_staging", ctypes.c_int, [c_void_p, ctypes.c_uint32]),
     ("nvc_prepare_hiz", ctypes.c_int, [c_void_p, ctypes.POINTER(HiZ)]),
     ("nvc_set_cluster_filter", ctypes.c_int, [c_void_p, ctypes.c_int]),

@@ -26,7 +26,7 @@ def _round_up(v, m):
 
 
 class VisibilityPath:
-    def __init__(self, meshes, meshlets, draws, depth_width, depth_height, device="cuda:0", task_wglimit=layout.TASK_WGLIMIT, cluster_limit=layout.CLUSTER_LIMIT, mesh_shading=True, hiz_stage_texels=None, prepare_meshes=True, prepare_hiz=True):
+    def __init__(self, meshes, meshlets, draws, depth_width, depth_height, device="cuda:0", task_wglimit=layout.TASK_WGLIMIT, cluster_limit=layout.CLUSTER_LIMIT, mesh_shading=True, hiz_stage_texels=None, prepare_meshes=True, prepare_meshlets=True, prepare_hiz=True):
         """meshes / meshlets / draws: structured numpy arrays (layout.MESH_DTYPE / MESHLET_DTYPE / MESHDRAW_DTYPE) or
         already-resident torch uint8 tensors.  draws must already carry meshletVisibilityOffset
         (host.visibility_offsets)."""
@@ -53,6 +53,9 @@ class VisibilityPath:
         if prepare_meshes:  # derived cull view of Mesh[] (once per geometry upload)
             mesh_count = self.mb.numel() // layout.MESH_DTYPE.itemsize
             check(self.lib.nvc_prepare_meshes(self.ctx, self._stream(), _ptr(self.mb), mesh_count), self.ctx, "nvc_prepare_meshes")
+        if prepare_meshlets:  # derived cull view of Meshlet[]: the 12 bytes the cluster passes read, as two dense arrays
+            meshlet_count = self.mlb.numel() // layout.MESHLET_DTYPE.itemsize
+            check(self.lib.nvc_prepare_meshlets(self.ctx, self._stream(), _ptr(self.mlb), meshlet_count), self.ctx, "nvc_prepare_meshlets")
 
         # niagara.cpp:1062-1090
         self.dvb = torch.zeros(max(1, self.draw_count), dtype=torch.int32, device=self.device)
