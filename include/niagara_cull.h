@@ -551,6 +551,35 @@ NVC_API int nvc_raster_depth(NvcContext* ctx, void* stream, const float* project
     const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words,
     const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4);
 
+/* The same depth producer in the task-shading submission mode (niagara.cpp:1666-1679: vkCmdDrawMeshTasksIndirectEXT(dccb, 4) ->
+ * meshlet.task.glsl EmitMeshTasksEXT(n, 1, 1) -> meshlet.mesh.glsl:94-103 with TASK = true): every command c < command_count4[1] * 64 of
+ * the (X, 64, 1) dispatch nvc_taskcull processed (padding commands included, X clamped to NVC_MAX_DISPATCH_GROUPS) launches
+ * n = min(emit_counts[c], 64) mesh workgroups (the clamp of the test driver's rs_mesh_payloads); workgroup i < n decodes
+ * ci = payloads[c].clusterIndices[i] exactly like nvc_raster_depth decodes a cib entry (~0 draws nothing, command = task_commands[ci & 0xffffff],
+ * meshlet = command.taskOffset + (ci >> 24)) and draws it with the same arithmetic, sampling and rejection rules.  payloads / emit_counts
+ * as written by nvc_taskcull.  stats4 (may be NULL, zeroed by the call): clusters drawn, triangles sampled, clusters rejected, depth
+ * updates issued.  Same bits as nvc_raster_depth over a cib holding the same cluster indices. */
+NVC_API int nvc_raster_depth_tasks(NvcContext* ctx, void* stream, const float* projection16, const NvcCullData* pass,
+    const NvcMeshTaskPayload* payloads, const uint32_t* emit_counts, const uint32_t* command_count4,
+    const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets,
+    const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices, uint32_t vertex_count,
+    float* depth, uint32_t width, uint32_t height, uint32_t* stats4);
+
+/* The same depth producer in the indexed-draw submission mode (mesh shading off, niagara.cpp:1680-1694:
+ * vkCmdDrawIndexedIndirectCount(dcb + 4, dccb, 0, maxDrawCount, 24) with mesh.vert.glsl:39-57): commands i < min(command_count4[0],
+ * max_draw_count) of draw_commands (written by nvc_drawcull(task = 0)); command i draws indexCount / 3 triangles from firstIndex
+ * (trailing indices that make no whole triangle are ignored); corner k of triangle t is vertex indices[firstIndex + 3t + k] + vertexOffset
+ * (uint32 wrap), transformed with draws[command.drawId] by mesh.vert's arithmetic (gl_DrawIDARB only selects the command).
+ * instanceCount == 0 draws nothing; instanceCount > 1 is drawn once (mesh.vert ignores gl_InstanceIndex and max is idempotent, so the
+ * image is the same).  A command whose [firstIndex, firstIndex + indexCount) is not inside indices[0, index_count) is skipped whole and
+ * counted; a triangle with a vertex >= vertex_count is skipped and counted; nothing is read outside the given arrays.  stats4 (may be
+ * NULL, zeroed by the call): commands drawn, triangles sampled, commands rejected, triangles rejected.  The image equals the test
+ * rasteriser's (oracle/refshader rs_draw_indexed) bit for bit. */
+NVC_API int nvc_raster_depth_indexed(NvcContext* ctx, void* stream, const float* projection16, const NvcCullData* pass,
+    const NvcMeshDrawCommand* draw_commands, const uint32_t* command_count4, uint32_t max_draw_count,
+    const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count,
+    float* depth, uint32_t width, uint32_t height, uint32_t* stats4);
+
 /* Recomputes center / radius / cone_axis / cone_cutoff of meshlets[0..meshlet_count) from geometry, bit-identical to
  * what the reference's cooker stores (scene.cpp:69-80 appendMeshlet -> meshopt_computeMeshletBounds,
  * meshletutils.cpp:133-272,314-339): one thread per meshlet reads its references and triangles from

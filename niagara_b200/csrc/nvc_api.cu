@@ -540,6 +540,36 @@ NVC_API int nvc_raster_depth(NvcContext* ctx, void* stream, const float* project
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_raster_depth");
 }
 
+NVC_API int nvc_raster_depth_tasks(NvcContext* ctx, void* stream, const float* projection16, const NvcCullData* pass, const NvcMeshTaskPayload* payloads, const uint32_t* emit_counts,
+    const uint32_t* command_count4, const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words,
+    const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4)
+{
+	if (!ctx || !projection16 || !pass || !payloads || !emit_counts || !command_count4 || !task_commands || !draws || !meshlets || !meshletdata || !vertices || !depth || width == 0 || height == 0)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (uint64_t(width) * height >= (1ull << 31))
+		return NVC_ERROR_UNSUPPORTED;
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	cudaError_t e = nvc::launch_raster_depth_tasks(projection16, *pass, payloads, emit_counts, command_count4, task_commands, draws, meshlets, meshletdata, meshletdata_words, vertices, vertex_count,
+	    depth, width, height, stats4, uint32_t(ctx->sm_count) * 16u, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_raster_depth_tasks");
+}
+
+NVC_API int nvc_raster_depth_indexed(NvcContext* ctx, void* stream, const float* projection16, const NvcCullData* pass, const NvcMeshDrawCommand* draw_commands, const uint32_t* command_count4,
+    uint32_t max_draw_count, const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height,
+    uint32_t* stats4)
+{
+	if (!ctx || !projection16 || !pass || !draw_commands || !command_count4 || !draws || !indices || !vertices || !depth || width == 0 || height == 0)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (uint64_t(width) * height >= (1ull << 31))
+		return NVC_ERROR_UNSUPPORTED;
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	cudaError_t e = nvc::launch_raster_depth_indexed(projection16, *pass, draw_commands, command_count4, max_draw_count, draws, indices, index_count, vertices, vertex_count, depth, width, height,
+	    stats4, uint32_t(ctx->sm_count) * 16u, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_raster_depth_indexed");
+}
+
 NVC_API int nvc_depth_pyramid(NvcContext* ctx, void* stream, const float* depth,
     uint32_t depth_width, uint32_t depth_height, const NvcHiZ* hiz)
 {

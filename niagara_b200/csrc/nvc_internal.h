@@ -200,6 +200,12 @@ cudaError_t launch_decode_clusters(const uint32_t* cluster_indices, const uint32
 cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pass, const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands,
     const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width,
     uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream);
+cudaError_t launch_raster_depth_tasks(const float* projection16, const NvcCullData& pass, const NvcMeshTaskPayload* payloads, const uint32_t* emit_counts, const uint32_t* command_count4,
+    const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices,
+    uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream);
+cudaError_t launch_raster_depth_indexed(const float* projection16, const NvcCullData& pass, const NvcMeshDrawCommand* draw_commands, const uint32_t* command_count4, uint32_t max_draw_count,
+    const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4,
+    uint32_t blocks, cudaStream_t stream);
 cudaError_t launch_cook_meshlet_bounds(const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* meshletdata, uint32_t meshletdata_words, NvcMeshlet* meshlets, uint32_t meshlet_count, uint32_t* rejected, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);

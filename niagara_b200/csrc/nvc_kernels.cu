@@ -1917,13 +1917,19 @@ cudaError_t launch_decode_clusters(const uint32_t* cluster_indices, const uint32
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Depth-only consumer of cib / ccb / dcb: what the reference's mesh stage + rasteriser do to the depth target between the
-// cull passes (niagara.cpp:1576-1701: vkCmdDrawMeshTasksIndirectEXT(ccb, 4) -> meshlet.mesh.glsl:89-206 -> fixed-function
-// raster, depth test GREATER on the reverse-Z buffer).  One warp per cluster slot: the lanes transform the <= 64 vertices
-// exactly as the mesh shader does (strict IEEE, GLSL operation order) into shared memory, then each lane rasterises its
-// share of the <= 96 triangles with the sampling rule of the test rasteriser (oracle/refshader/driver.cpp rasterTriangle:
-// pixel centres, edge functions and depth interpolation in binary64, back faces / w <= 0 dropped) and merges depth with
-// atomicMax — max is order independent, so the image is bit-identical to the sequential CPU rasteriser's.
+// Depth-only consumers of the cull output: what the reference's mesh / vertex stage + rasteriser do to the depth target between the
+// cull passes (niagara.cpp:1576-1701, fixed-function raster, depth test GREATER on the reverse-Z buffer), in its three submission
+// modes:
+//   cluster submit  vkCmdDrawMeshTasksIndirectEXT(ccb, 4) -> meshlet.mesh.glsl:89-206 over cib       raster_clusters_kernel<false>
+//   task shading    vkCmdDrawMeshTasksIndirectEXT(dccb, 4) -> meshlet.task EmitMeshTasksEXT(n) ->
+//                   meshlet.mesh.glsl (TASK = true) over the task payloads                            raster_clusters_kernel<true>
+//   indexed draws   vkCmdDrawIndexedIndirectCount(dcb + 4, dccb, 0, maxDrawCount, 24) -> mesh.vert    raster_indexed_kernel
+// Cluster modes: one warp per cluster; the lanes transform the <= 64 vertices exactly as the mesh shader does (strict IEEE, GLSL
+// operation order) into shared memory, then each lane rasterises its share of the <= 96 triangles.  Indexed mode: one warp per
+// 1/32 of a command's triangles, each lane transforms the three corners of its triangles (mesh.vert's arithmetic is the mesh shader's).  Every triangle
+// is sampled with the rule of the test rasteriser (oracle/refshader/driver.cpp rasterTriangle: pixel centres, edge functions and
+// depth interpolation in binary64, back faces / w <= 0 dropped) and merged with atomicMax — max is order independent, so the image
+// is bit-identical to the sequential CPU rasteriser's.
 // This is what lets the two-phase path run on PRODUCED depth on the device (BASELINE configs[2]).
 // ------------------------------------------------------------------------------------------------------
 constexpr int kRasterWarps = 4;
@@ -1939,13 +1945,117 @@ __device__ __forceinline__ float4 mat4_mul_vec4(const float* __restrict__ m, flo
 	return r;
 }
 
+// Clip position of vertices[vi] under the draw (d0 = position.xyz, scale; d1 = orientation): meshlet.mesh.glsl:127-140 ==
+// mesh.vert.glsl:44-57, rotateQuat(position) * scale + position, then projection * (view * vec4(wpos, 1)).
+__device__ __forceinline__ float4 transform_vertex(const NvcVertex* vertices, uint32_t vi, float4 d0, float4 d1, const float* view, const float* projection)
+{
+	const uint2 vv = __ldg(reinterpret_cast<const uint2*>(vertices + vi)); // vx, vy | vz, tp
+	f3 pos = { half_bits_to_float(vv.x & 0xffffu), half_bits_to_float(vv.x >> 16), half_bits_to_float(vv.y & 0xffffu) };
+	f3 r = rotate_quat(pos, d1);
+	const float wx = __fadd_rn(__fmul_rn(r.x, d0.w), d0.x), wy = __fadd_rn(__fmul_rn(r.y, d0.w), d0.y), wz = __fadd_rn(__fmul_rn(r.z, d0.w), d0.z);
+	const float4 v = mat4_mul_vec4(view, wx, wy, wz, 1.0f);
+	return mat4_mul_vec4(projection, v.x, v.y, v.z, v.w);
+}
+
+// One triangle given as three clip-space corners, sampled into depth[height][width] with max (driver.cpp rasterTriangle).
+// tris counts triangles that reach sampling, writes the depth updates issued.
+__device__ __forceinline__ void raster_triangle(const float4 (&pc)[3], float* depth, uint32_t width, uint32_t height, double fw, double fh, uint32_t& tris, uint32_t& writes)
+{
+	double sx[3], sy[3], sz[3];
+	bool front = true;
+#pragma unroll
+	for (int c = 0; c < 3; ++c)
+	{
+		front = front && pc[c].w > 0.0f;
+		const float fx = __fmul_rn(__fadd_rn(__fmul_rn(__fdiv_rn(pc[c].x, pc[c].w), 0.5f), 0.5f), float(width));
+		const float fy = __fmul_rn(__fadd_rn(__fmul_rn(__fdiv_rn(pc[c].y, pc[c].w), 0.5f), 0.5f), float(height));
+		sx[c] = double(fx);
+		sy[c] = double(fy);
+		sz[c] = double(__fdiv_rn(pc[c].z, pc[c].w));
+	}
+	if (!front)
+		return;
+	const double ebx = __dsub_rn(sx[1], sx[0]), eby = __dsub_rn(sy[1], sy[0]), ecx = __dsub_rn(sx[2], sx[0]), ecy = __dsub_rn(sy[2], sy[0]);
+	const double area = __dsub_rn(__dmul_rn(ebx, ecy), __dmul_rn(eby, ecx));
+	if (!(area > 0.0))
+		return; // back facing or zero area
+	// flipped viewport: rows count from the top; swapping two corners keeps the edge functions positive inside
+#pragma unroll
+	for (int c = 0; c < 3; ++c)
+		sy[c] = __dsub_rn(fh, sy[c]);
+	{
+		double tx = sx[1], ty = sy[1], tz = sz[1];
+		sx[1] = sx[2], sy[1] = sy[2], sz[1] = sz[2];
+		sx[2] = tx, sy[2] = ty, sz[2] = tz;
+	}
+	const double minx = fmin(sx[0], fmin(sx[1], sx[2])), maxx = fmax(sx[0], fmax(sx[1], sx[2]));
+	const double miny = fmin(sy[0], fmin(sy[1], sy[2])), maxy = fmax(sy[0], fmax(sy[1], sy[2]));
+	if (!(maxx >= 0.0 && maxy >= 0.0 && minx <= fw && miny <= fh))
+		return;
+	const int x0 = int(fmax(0.0, floor(__dsub_rn(minx, 0.5)))), x1 = int(fmin(__dsub_rn(fw, 1.0), ceil(__dsub_rn(maxx, 0.5))));
+	const int y0 = int(fmax(0.0, floor(__dsub_rn(miny, 0.5)))), y1 = int(fmin(__dsub_rn(fh, 1.0), ceil(__dsub_rn(maxy, 0.5))));
+	++tris;
+	for (int yy = y0; yy <= y1; ++yy)
+		for (int xx = x0; xx <= x1; ++xx)
+		{
+			const double px = __dadd_rn(double(xx), 0.5), py = __dadd_rn(double(yy), 0.5);
+			const double w0 = __dsub_rn(__dmul_rn(__dsub_rn(sx[1], px), __dsub_rn(sy[2], py)), __dmul_rn(__dsub_rn(sy[1], py), __dsub_rn(sx[2], px)));
+			const double w1 = __dsub_rn(__dmul_rn(__dsub_rn(sx[2], px), __dsub_rn(sy[0], py)), __dmul_rn(__dsub_rn(sy[2], py), __dsub_rn(sx[0], px)));
+			const double w2 = __dsub_rn(__dmul_rn(__dsub_rn(sx[0], px), __dsub_rn(sy[1], py)), __dmul_rn(__dsub_rn(sy[0], py), __dsub_rn(sx[1], px)));
+			if (w0 < 0.0 || w1 < 0.0 || w2 < 0.0)
+				continue;
+			const double num = __dadd_rn(__dadd_rn(__dmul_rn(w0, sz[0]), __dmul_rn(w1, sz[1])), __dmul_rn(w2, sz[2]));
+			const double den = __dadd_rn(__dadd_rn(w0, w1), w2);
+			const float zf = float(__ddiv_rn(num, den));
+			// depth test GREATER on a buffer cleared to 0: only positive, ordered values can win; for those the float
+			// order is the order of their bit patterns
+			if (zf > 0.0f)
+			{
+				atomicMax(reinterpret_cast<int*>(depth) + size_t(yy) * width + xx, __float_as_int(zf));
+				++writes;
+			}
+		}
+}
+
+// warp-reduces the four per-lane counters and adds them to stats4 (nullptr: not wanted)
+__device__ __forceinline__ void flush_stats4(uint32_t* stats4, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3)
+{
+	if (!stats4)
+		return;
+#pragma unroll
+	for (int o = 16; o >= 1; o >>= 1)
+	{
+		s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+		s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+		s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+		s3 += __shfl_xor_sync(0xffffffffu, s3, o);
+	}
+	if (lane_id() == 0)
+	{
+		if (s0)
+			atomicAdd(stats4 + 0, s0);
+		if (s1)
+			atomicAdd(stats4 + 1, s1);
+		if (s2)
+			atomicAdd(stats4 + 2, s2);
+		if (s3)
+			atomicAdd(stats4 + 3, s3);
+	}
+}
+
 struct RasterParams
 {
 	float projection[16];
 	float view[16];
-	const uint32_t* cluster_indices;
-	const uint32_t* cluster_count4;
+	const uint32_t* cluster_indices; // cluster submit: cib
+	const uint32_t* cluster_count4;  // cluster submit: ccb
+	const NvcMeshTaskPayload* payloads; // task shading: payloads[c], emit_counts[c] for c < command_count4[1] * 64
+	const uint32_t* emit_counts;
+	const uint32_t* command_count4; // task shading / indexed draws: dccb
 	const NvcMeshTaskCommand* task_commands;
+	const NvcMeshDrawCommand* draw_commands; // indexed draws: dcb, indices[index_count]
+	const uint32_t* indices;
+	uint32_t index_count, max_draw_count;
 	const NvcMeshDraw* draws;
 	const NvcMeshlet* meshlets;
 	const uint32_t* meshletdata;
@@ -1954,24 +2064,48 @@ struct RasterParams
 	uint32_t vertex_count;
 	float* depth;
 	uint32_t width, height;
-	uint32_t* stats4; // clusters drawn, triangles rasterised, clusters rejected (data out of range), pixels written (approximate: updates)
+	// clusters / commands drawn, triangles rasterised, clusters / commands rejected (data out of range), cluster modes: depth
+	// updates issued, indexed draws: triangles rejected (vertex index out of range)
+	uint32_t* stats4;
 };
 
-__global__ void __launch_bounds__(kRasterWarps * 32) raster_depth_kernel(const RasterParams p)
+// Task = false: work item w is slot x + y * 256 + z * 16 of the (16, Y, 16) dispatch in ccb, reading cib (meshlet.mesh.glsl:94).
+// Task = true: work item w is mesh workgroup i = w % 64 of task command c = w / 64 of the (X, 64, 1) dispatch in dccb; it exists when
+// i < min(emit_counts[c], 64) and reads payloads[c].clusterIndices[i].  Everything after the cluster index is the same code.
+template <bool Task>
+__global__ void __launch_bounds__(kRasterWarps * 32) raster_clusters_kernel(const RasterParams p)
 {
 	__shared__ float4 s_clip[kRasterWarps][64];
 	const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
-	const uint32_t gx = p.cluster_count4[1], gy = p.cluster_count4[2], gz = p.cluster_count4[3];
-	const uint32_t slots = gx * gy * gz;
+	uint32_t gx = 0, gz = 0, items;
+	if (Task)
+		items = min(p.command_count4[1], NVC_MAX_DISPATCH_GROUPS) * NVC_TASK_WGSIZE * NVC_TASK_WGSIZE;
+	else
+	{
+		gx = p.cluster_count4[1];
+		gz = p.cluster_count4[3];
+		items = gx * p.cluster_count4[2] * gz;
+	}
 	float4* clip = s_clip[warp];
 	uint32_t drawn = 0, tris = 0, rejected = 0, writes = 0;
 	const double fw = double(p.width), fh = double(p.height);
 
-	for (uint32_t w = blockIdx.x * kRasterWarps + warp; w < slots; w += gridDim.x * kRasterWarps)
+	for (uint32_t w = blockIdx.x * kRasterWarps + warp; w < items; w += gridDim.x * kRasterWarps)
 	{
-		const uint32_t x = w % gx, z = (w / gx) % gz, y = w / (gx * gz);
-		const uint32_t slot = x + y * 256u + z * NVC_CLUSTER_TILE; // meshlet.mesh.glsl:94
-		const uint32_t ci = __ldg(p.cluster_indices + slot);
+		uint32_t ci;
+		if (Task)
+		{
+			const uint32_t c = w / NVC_TASK_WGSIZE, i = w % NVC_TASK_WGSIZE;
+			if (i >= min(__ldg(p.emit_counts + c), NVC_TASK_WGSIZE))
+				continue; // EmitMeshTasksEXT(n) launched no such workgroup
+			ci = __ldg(p.payloads[c].clusterIndices + i);
+		}
+		else
+		{
+			const uint32_t x = w % gx, z = (w / gx) % gz, y = w / (gx * gz);
+			const uint32_t slot = x + y * 256u + z * NVC_CLUSTER_TILE; // meshlet.mesh.glsl:94
+			ci = __ldg(p.cluster_indices + slot);
+		}
 		if (ci == ~0u)
 			continue; // SetMeshOutputsEXT(0, 0)
 		const uint32_t* cp = reinterpret_cast<const uint32_t*>(p.task_commands + (ci & 0xffffffu));
@@ -2002,12 +2136,7 @@ __global__ void __launch_bounds__(kRasterWarps * 32) raster_depth_kernel(const R
 				bad = true;
 				break;
 			}
-			const uint2 vv = __ldg(reinterpret_cast<const uint2*>(p.vertices + vi)); // vx, vy | vz, tp
-			f3 pos = { half_bits_to_float(vv.x & 0xffffu), half_bits_to_float(vv.x >> 16), half_bits_to_float(vv.y & 0xffffu) };
-			f3 r = rotate_quat(pos, d1);
-			const float wx = __fadd_rn(__fmul_rn(r.x, d0.w), d0.x), wy = __fadd_rn(__fmul_rn(r.y, d0.w), d0.y), wz = __fadd_rn(__fmul_rn(r.z, d0.w), d0.z);
-			const float4 v = mat4_mul_vec4(p.view, wx, wy, wz, 1.0f);
-			clip[i] = mat4_mul_vec4(p.projection, v.x, v.y, v.z, v.w);
+			clip[i] = transform_vertex(p.vertices, vi, d0, d1, p.view, p.projection);
 		}
 		if (__any_sync(0xffffffffu, bad))
 		{
@@ -2026,115 +2155,141 @@ __global__ void __launch_bounds__(kRasterWarps * 32) raster_depth_kernel(const R
 			if (ia >= vertexCount || ib >= vertexCount || ic >= vertexCount)
 				continue;
 			const float4 pc[3] = { clip[ia], clip[ib], clip[ic] };
-			double sx[3], sy[3], sz[3];
-			bool front = true;
-#pragma unroll
-			for (int c = 0; c < 3; ++c)
-			{
-				front = front && pc[c].w > 0.0f;
-				const float fx = __fmul_rn(__fadd_rn(__fmul_rn(__fdiv_rn(pc[c].x, pc[c].w), 0.5f), 0.5f), float(p.width));
-				const float fy = __fmul_rn(__fadd_rn(__fmul_rn(__fdiv_rn(pc[c].y, pc[c].w), 0.5f), 0.5f), float(p.height));
-				sx[c] = double(fx);
-				sy[c] = double(fy);
-				sz[c] = double(__fdiv_rn(pc[c].z, pc[c].w));
-			}
-			if (!front)
-				continue;
-			const double ebx = __dsub_rn(sx[1], sx[0]), eby = __dsub_rn(sy[1], sy[0]), ecx = __dsub_rn(sx[2], sx[0]), ecy = __dsub_rn(sy[2], sy[0]);
-			const double area = __dsub_rn(__dmul_rn(ebx, ecy), __dmul_rn(eby, ecx));
-			if (!(area > 0.0))
-				continue; // back facing or zero area
-			// flipped viewport: rows count from the top; swapping two corners keeps the edge functions positive inside
-#pragma unroll
-			for (int c = 0; c < 3; ++c)
-				sy[c] = __dsub_rn(fh, sy[c]);
-			{
-				double tx = sx[1], ty = sy[1], tz = sz[1];
-				sx[1] = sx[2], sy[1] = sy[2], sz[1] = sz[2];
-				sx[2] = tx, sy[2] = ty, sz[2] = tz;
-			}
-			const double minx = fmin(sx[0], fmin(sx[1], sx[2])), maxx = fmax(sx[0], fmax(sx[1], sx[2]));
-			const double miny = fmin(sy[0], fmin(sy[1], sy[2])), maxy = fmax(sy[0], fmax(sy[1], sy[2]));
-			if (!(maxx >= 0.0 && maxy >= 0.0 && minx <= fw && miny <= fh))
-				continue;
-			const int x0 = int(fmax(0.0, floor(__dsub_rn(minx, 0.5)))), x1 = int(fmin(__dsub_rn(fw, 1.0), ceil(__dsub_rn(maxx, 0.5))));
-			const int y0 = int(fmax(0.0, floor(__dsub_rn(miny, 0.5)))), y1 = int(fmin(__dsub_rn(fh, 1.0), ceil(__dsub_rn(maxy, 0.5))));
-			++tris;
-			for (int yy = y0; yy <= y1; ++yy)
-				for (int xx = x0; xx <= x1; ++xx)
-				{
-					const double px = __dadd_rn(double(xx), 0.5), py = __dadd_rn(double(yy), 0.5);
-					const double w0 = __dsub_rn(__dmul_rn(__dsub_rn(sx[1], px), __dsub_rn(sy[2], py)), __dmul_rn(__dsub_rn(sy[1], py), __dsub_rn(sx[2], px)));
-					const double w1 = __dsub_rn(__dmul_rn(__dsub_rn(sx[2], px), __dsub_rn(sy[0], py)), __dmul_rn(__dsub_rn(sy[2], py), __dsub_rn(sx[0], px)));
-					const double w2 = __dsub_rn(__dmul_rn(__dsub_rn(sx[0], px), __dsub_rn(sy[1], py)), __dmul_rn(__dsub_rn(sy[0], py), __dsub_rn(sx[1], px)));
-					if (w0 < 0.0 || w1 < 0.0 || w2 < 0.0)
-						continue;
-					const double num = __dadd_rn(__dadd_rn(__dmul_rn(w0, sz[0]), __dmul_rn(w1, sz[1])), __dmul_rn(w2, sz[2]));
-					const double den = __dadd_rn(__dadd_rn(w0, w1), w2);
-					const float zf = float(__ddiv_rn(num, den));
-					// depth test GREATER on a buffer cleared to 0: only positive, ordered values can win; for those the float
-					// order is the order of their bit patterns
-					if (zf > 0.0f)
-					{
-						atomicMax(reinterpret_cast<int*>(p.depth) + size_t(yy) * p.width + xx, __float_as_int(zf));
-						++writes;
-					}
-				}
+			raster_triangle(pc, p.depth, p.width, p.height, fw, fh, tris, writes);
 		}
 		__syncwarp(); // the next cluster reuses clip[]
 	}
-	if (p.stats4)
-	{
-#pragma unroll
-		for (int o = 16; o >= 1; o >>= 1)
-		{
-			drawn += __shfl_xor_sync(0xffffffffu, drawn, o);
-			tris += __shfl_xor_sync(0xffffffffu, tris, o);
-			rejected += __shfl_xor_sync(0xffffffffu, rejected, o);
-			writes += __shfl_xor_sync(0xffffffffu, writes, o);
-		}
-		if (lane == 0)
-		{
-			if (drawn)
-				atomicAdd(p.stats4 + 0, drawn);
-			if (tris)
-				atomicAdd(p.stats4 + 1, tris);
-			if (rejected)
-				atomicAdd(p.stats4 + 2, rejected);
-			if (writes)
-				atomicAdd(p.stats4 + 3, writes);
-		}
-	}
+	flush_stats4(p.stats4, drawn, tris, rejected, writes);
 }
 
-cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pass, const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands,
-    const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width,
-    uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream)
+// Commands i < min(command_count4[0], max_draw_count) of dcb, each split into kIndexedSlices equal runs of its indexCount / 3
+// triangles; one warp per (command, run) (grid-stride), the lanes striding over the run.  Corner k of triangle t is vertex
+// indices[firstIndex + 3t + k] + vertexOffset (uint32 wrap) under draws[drawId] (gl_DrawIDARB only selects the command).
+// mesh.vert ignores gl_InstanceIndex and max is idempotent, so a command with instanceCount >= 1 is drawn once and one with
+// instanceCount == 0 draws nothing.
+// One warp per whole command was 8x slower than cluster submit on the C3 stand-in (H100, 23 ms against 2.9 ms for the early
+// pass): a close LOD-0 kitten (28 944 triangles) kept a single warp busy for the whole pass.
+constexpr uint32_t kIndexedSlices = 32;
+
+__global__ void __launch_bounds__(kRasterWarps * 32) raster_indexed_kernel(const RasterParams p)
+{
+	const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
+	const uint64_t items = uint64_t(min(p.command_count4[0], p.max_draw_count)) * kIndexedSlices;
+	uint32_t drawn = 0, tris = 0, rejected = 0, bad_tris = 0, writes = 0;
+	const double fw = double(p.width), fh = double(p.height);
+
+	for (uint64_t w = blockIdx.x * kRasterWarps + warp; w < items; w += gridDim.x * kRasterWarps)
+	{
+		const uint32_t slice = uint32_t(w % kIndexedSlices);
+		const uint32_t* cp = reinterpret_cast<const uint32_t*>(p.draw_commands + w / kIndexedSlices);
+		const uint32_t drawId = __ldg(cp + 0), indexCount = __ldg(cp + 1), instanceCount = __ldg(cp + 2);
+		const uint32_t firstIndex = __ldg(cp + 3), vertexOffset = __ldg(cp + 4);
+		if (instanceCount == 0)
+			continue;
+		if (uint64_t(firstIndex) + indexCount > p.index_count)
+		{
+			rejected += lane == 0 && slice == 0;
+			continue;
+		}
+		drawn += lane == 0 && slice == 0;
+		const uint32_t triangles = indexCount / 3; // trailing indices that make no whole triangle are not drawn
+		const uint32_t run = (triangles + kIndexedSlices - 1) / kIndexedSlices;
+		const uint32_t t_end = min(triangles, slice * run + run);
+		if (slice * run >= t_end)
+			continue;
+		const char* dp = reinterpret_cast<const char*>(p.draws + drawId);
+		const float4 d0 = ldg_f4(dp), d1 = ldg_f4(dp + 16);
+		const uint32_t* idx = p.indices + firstIndex;
+		for (uint32_t t = slice * run + lane; t < t_end; t += 32)
+		{
+			const uint32_t va = __ldg(idx + size_t(t) * 3 + 0) + vertexOffset, vb = __ldg(idx + size_t(t) * 3 + 1) + vertexOffset, vc = __ldg(idx + size_t(t) * 3 + 2) + vertexOffset;
+			if (va >= p.vertex_count || vb >= p.vertex_count || vc >= p.vertex_count)
+			{
+				++bad_tris;
+				continue;
+			}
+			const float4 pc[3] = { transform_vertex(p.vertices, va, d0, d1, p.view, p.projection), transform_vertex(p.vertices, vb, d0, d1, p.view, p.projection),
+				transform_vertex(p.vertices, vc, d0, d1, p.view, p.projection) };
+			raster_triangle(pc, p.depth, p.width, p.height, fw, fh, tris, writes);
+		}
+	}
+	flush_stats4(p.stats4, drawn, tris, rejected, bad_tris);
+}
+
+namespace
+{
+
+RasterParams raster_params(const float* projection16, const NvcCullData& pass, const NvcMeshDraw* draws, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width,
+    uint32_t height, uint32_t* stats4)
 {
 	RasterParams p;
+	memset(&p, 0, sizeof(p));
 	memcpy(p.projection, projection16, sizeof(p.projection));
 	memcpy(p.view, pass.view, sizeof(p.view));
-	p.cluster_indices = cluster_indices;
-	p.cluster_count4 = cluster_count4;
-	p.task_commands = task_commands;
 	p.draws = draws;
-	p.meshlets = meshlets;
-	p.meshletdata = meshletdata;
-	p.meshletdata_words = meshletdata_words;
 	p.vertices = vertices;
 	p.vertex_count = vertex_count;
 	p.depth = depth;
 	p.width = width;
 	p.height = height;
 	p.stats4 = stats4;
-	if (stats4)
+	return p;
+}
+
+cudaError_t launch_raster(void (*kernel)(RasterParams), const RasterParams& p, uint32_t blocks, cudaStream_t stream)
+{
+	if (p.stats4)
 	{
-		cudaError_t e = cudaMemsetAsync(stats4, 0, 16, stream);
+		cudaError_t e = cudaMemsetAsync(p.stats4, 0, 16, stream);
 		if (e != cudaSuccess)
 			return e;
 	}
-	raster_depth_kernel<<<blocks, kRasterWarps * 32, 0, stream>>>(p);
+	kernel<<<blocks, kRasterWarps * 32, 0, stream>>>(p);
 	return cudaGetLastError();
+}
+
+} // namespace
+
+cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pass, const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands,
+    const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width,
+    uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream)
+{
+	RasterParams p = raster_params(projection16, pass, draws, vertices, vertex_count, depth, width, height, stats4);
+	p.cluster_indices = cluster_indices;
+	p.cluster_count4 = cluster_count4;
+	p.task_commands = task_commands;
+	p.meshlets = meshlets;
+	p.meshletdata = meshletdata;
+	p.meshletdata_words = meshletdata_words;
+	return launch_raster(raster_clusters_kernel<false>, p, blocks, stream);
+}
+
+cudaError_t launch_raster_depth_tasks(const float* projection16, const NvcCullData& pass, const NvcMeshTaskPayload* payloads, const uint32_t* emit_counts, const uint32_t* command_count4,
+    const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices,
+    uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream)
+{
+	RasterParams p = raster_params(projection16, pass, draws, vertices, vertex_count, depth, width, height, stats4);
+	p.payloads = payloads;
+	p.emit_counts = emit_counts;
+	p.command_count4 = command_count4;
+	p.task_commands = task_commands;
+	p.meshlets = meshlets;
+	p.meshletdata = meshletdata;
+	p.meshletdata_words = meshletdata_words;
+	return launch_raster(raster_clusters_kernel<true>, p, blocks, stream);
+}
+
+cudaError_t launch_raster_depth_indexed(const float* projection16, const NvcCullData& pass, const NvcMeshDrawCommand* draw_commands, const uint32_t* command_count4, uint32_t max_draw_count,
+    const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4,
+    uint32_t blocks, cudaStream_t stream)
+{
+	RasterParams p = raster_params(projection16, pass, draws, vertices, vertex_count, depth, width, height, stats4);
+	p.draw_commands = draw_commands;
+	p.command_count4 = command_count4;
+	p.max_draw_count = max_draw_count;
+	p.indices = indices;
+	p.index_count = index_count;
+	return launch_raster(raster_indexed_kernel, p, blocks, stream);
 }
 
 // N4: meshlet bounds + normal cone, one thread per meshlet (csrc/nvc_cook.cuh).  A meshlet whose data or vertices would

@@ -170,6 +170,30 @@ class VisibilityPath:
             "nvc_raster_depth",
         )
 
+    def raster_depth_tasks(self, cull_data, projection16, payloads, emit_counts, vertices, meshletdata, depth, stats=None):
+        """raster_depth in the task-shading mode (nvc_raster_depth_tasks): draws the clusters that task_shading() put into
+        payloads / emit_counts for this path's dcb / dccb."""
+        pass_data = layout.CullData()
+        self.lib.nvc_host_pass_data(ctypes.byref(cull_data), 0, 0, ctypes.byref(pass_data))
+        proj = (ctypes.c_float * 16)(*[float(v) for v in projection16])
+        check(
+            self.lib.nvc_raster_depth_tasks(self.ctx, self._stream(), proj, ctypes.byref(pass_data), _ptr(payloads), _ptr(emit_counts), _ptr(self.dccb), _ptr(self.dcb), _ptr(self.db), _ptr(self.mlb), _ptr(meshletdata), meshletdata.numel(), _ptr(vertices), vertices.numel() // 16, _ptr(depth), depth.shape[1], depth.shape[0], _ptr(stats)),
+            self.ctx,
+            "nvc_raster_depth_tasks",
+        )
+
+    def raster_depth_indexed(self, cull_data, projection16, vertices, indices, depth, stats=None):
+        """raster_depth in the indexed-draw mode (nvc_raster_depth_indexed): draws this path's MeshDrawCommand[] (cull(task=False))
+        with max_draw_count = draw_count.  indices: int32 device tensor of the uint32 index buffer."""
+        pass_data = layout.CullData()
+        self.lib.nvc_host_pass_data(ctypes.byref(cull_data), 0, 0, ctypes.byref(pass_data))
+        proj = (ctypes.c_float * 16)(*[float(v) for v in projection16])
+        check(
+            self.lib.nvc_raster_depth_indexed(self.ctx, self._stream(), proj, ctypes.byref(pass_data), _ptr(self.dcb), _ptr(self.dccb), self.draw_count, _ptr(self.db), _ptr(indices), indices.numel(), _ptr(vertices), vertices.numel() // 16, _ptr(depth), depth.shape[1], depth.shape[0], _ptr(stats)),
+            self.ctx,
+            "nvc_raster_depth_indexed",
+        )
+
     def frame(self, cull_data, depth, post_passes=False, cluster_backface=None):
         """One frame of the hot path in the reference's order (niagara.cpp:1765-1788).  `depth` stands in for the
         depth target the early render would have produced."""
