@@ -580,6 +580,17 @@ NVC_API int nvc_raster_depth_indexed(NvcContext* ctx, void* stream, const float*
     const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count,
     float* depth, uint32_t width, uint32_t height, uint32_t* stats4);
 
+/* meshlet.mesh.glsl with MESH_CULL = 1 (config.h:11; the reference default is 0): nvc_raster_depth and nvc_raster_depth_tasks
+ * enqueued after this call drop the triangles the mesh shader marks gl_CullPrimitiveEXT (meshlet.mesh.glsl:175-195: back-facing and
+ * zero-area triangles, and triangles whose screen bounding box rounds to a single column or row, when all three corners have w > 0;
+ * `round` is half away from zero).  A culled triangle is not sampled, so stats4[1] (triangles sampled) gets smaller; the other
+ * statistics keep their meaning.  nvc_raster_depth_indexed is not affected (mesh.vert has no such stage).  Default 0.  The setting
+ * is read when a call is enqueued: a captured graph keeps the value that was current at capture time. */
+NVC_API int nvc_set_mesh_cull(NvcContext* ctx, int enabled);
+/* Diagnostics (synchronises the device): out[0] = triangles the mesh-cull stage tested, out[1] = how many it culled, both
+ * cumulative since the last call with reset != 0. */
+NVC_API int nvc_mesh_cull_stats(NvcContext* ctx, uint64_t* out_tested_culled2, int reset);
+
 /* Recomputes center / radius / cone_axis / cone_cutoff of meshlets[0..meshlet_count) from geometry, bit-identical to
  * what the reference's cooker stores (scene.cpp:69-80 appendMeshlet -> meshopt_computeMeshletBounds,
  * meshletutils.cpp:133-272,314-339): one thread per meshlet reads its references and triangles from

@@ -525,6 +525,41 @@ NVC_API int nvc_decode_clusters(NvcContext* ctx, void* stream, const uint32_t* c
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_decode_clusters");
 }
 
+// the mesh-cull counters when the stage is on (read when the call is enqueued), nullptr when it is off
+static unsigned long long* mesh_cull_counters(NvcContext* ctx)
+{
+	return ctx->mesh_cull ? &ctx->scratch->mesh_cull_tested : nullptr;
+}
+
+NVC_API int nvc_set_mesh_cull(NvcContext* ctx, int enabled)
+{
+	if (!ctx)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	ctx->mesh_cull = enabled != 0;
+	return NVC_OK;
+}
+
+NVC_API int nvc_mesh_cull_stats(NvcContext* ctx, uint64_t* out_tested_culled2, int reset)
+{
+	if (!ctx)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	DeviceGuard guard(ctx->device);
+	cudaError_t e = cudaDeviceSynchronize();
+	unsigned long long v[2] = { 0, 0 };
+	if (e == cudaSuccess)
+		e = cudaMemcpy(v, &ctx->scratch->mesh_cull_tested, sizeof(v), cudaMemcpyDeviceToHost);
+	if (e == cudaSuccess && reset)
+		e = cudaMemset(&ctx->scratch->mesh_cull_tested, 0, sizeof(v));
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, "nvc_mesh_cull_stats");
+	if (out_tested_culled2)
+	{
+		out_tested_culled2[0] = v[0];
+		out_tested_culled2[1] = v[1];
+	}
+	return NVC_OK;
+}
+
 NVC_API int nvc_raster_depth(NvcContext* ctx, void* stream, const float* projection16, const NvcCullData* pass, const uint32_t* cluster_indices, const uint32_t* cluster_count4,
     const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices,
     uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4)
@@ -536,7 +571,7 @@ NVC_API int nvc_raster_depth(NvcContext* ctx, void* stream, const float* project
 	if (!device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	cudaError_t e = nvc::launch_raster_depth(projection16, *pass, cluster_indices, cluster_count4, task_commands, draws, meshlets, meshletdata, meshletdata_words, vertices, vertex_count, depth,
-	    width, height, stats4, uint32_t(ctx->sm_count) * 16u, static_cast<cudaStream_t>(stream));
+	    width, height, stats4, mesh_cull_counters(ctx), uint32_t(ctx->sm_count) * 16u, static_cast<cudaStream_t>(stream));
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_raster_depth");
 }
 
@@ -551,7 +586,7 @@ NVC_API int nvc_raster_depth_tasks(NvcContext* ctx, void* stream, const float* p
 	if (!device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	cudaError_t e = nvc::launch_raster_depth_tasks(projection16, *pass, payloads, emit_counts, command_count4, task_commands, draws, meshlets, meshletdata, meshletdata_words, vertices, vertex_count,
-	    depth, width, height, stats4, uint32_t(ctx->sm_count) * 16u, static_cast<cudaStream_t>(stream));
+	    depth, width, height, stats4, mesh_cull_counters(ctx), uint32_t(ctx->sm_count) * 16u, static_cast<cudaStream_t>(stream));
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_raster_depth_tasks");
 }
 

@@ -21,6 +21,7 @@ struct NvcContext
 	int cluster_filter_blocks_early = 0, cluster_filter_blocks_late = 0;
 	bool draw_filter = false;   // env NVC_DRAW_FILTER=1: filtered occlusion stage of the late drawcull (off by default: the pass is not issue bound)
 	bool cluster_filter = true; // nvc_set_cluster_filter / env NVC_CLUSTER_FILTER: filtered cluster kernel (default) or the exact one
+	bool mesh_cull = false;     // nvc_set_mesh_cull: the mesh shader's per-triangle cull stage (MESH_CULL) in the cluster-mode depth producers
 	uint32_t hiz_stage_budget = 0; // texels (24 KB) of coarse Hi-Z mips staged per CTA; 0 = off (env NVC_HIZ_STAGE_TEXELS)
 	NvcLimits limits = { NVC_TASK_WGLIMIT, NVC_CLUSTER_LIMIT };
 	nvc::Scratch* scratch = nullptr;
@@ -73,6 +74,10 @@ struct alignas(128) Scratch
 	// filtered cluster pass, cumulative since the last nvc_filter_stats(reset): meshlets evaluated, meshlets that took the exact path
 	unsigned long long filter_items, filter_undecided;
 	uint32_t pad6[28];
+	// mesh-cull stage of the depth producers (nvc_set_mesh_cull), cumulative since the last nvc_mesh_cull_stats(reset): triangles
+	// tested, triangles culled
+	unsigned long long mesh_cull_tested, mesh_cull_culled;
+	uint32_t pad7[28];
 };
 
 // row pitch of a footprint-image level of width w (w + 1 entries per row, padded so that every row starts 16-byte aligned)
@@ -199,10 +204,10 @@ cudaError_t launch_footprint(const HiZDesc& hiz, float* fp, uint32_t total, cuda
 cudaError_t launch_decode_clusters(const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands, const NvcMeshlet* meshlets, NvcClusterRecord* records, uint32_t* stats4, uint32_t blocks, cudaStream_t stream);
 cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pass, const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands,
     const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width,
-    uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream);
+    uint32_t height, uint32_t* stats4, unsigned long long* mesh_cull2, uint32_t blocks, cudaStream_t stream);
 cudaError_t launch_raster_depth_tasks(const float* projection16, const NvcCullData& pass, const NvcMeshTaskPayload* payloads, const uint32_t* emit_counts, const uint32_t* command_count4,
     const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices,
-    uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream);
+    uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4, unsigned long long* mesh_cull2, uint32_t blocks, cudaStream_t stream);
 cudaError_t launch_raster_depth_indexed(const float* projection16, const NvcCullData& pass, const NvcMeshDrawCommand* draw_commands, const uint32_t* command_count4, uint32_t max_draw_count,
     const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4,
     uint32_t blocks, cudaStream_t stream);

@@ -1920,9 +1920,10 @@ cudaError_t launch_decode_clusters(const uint32_t* cluster_indices, const uint32
 // Depth-only consumers of the cull output: what the reference's mesh / vertex stage + rasteriser do to the depth target between the
 // cull passes (niagara.cpp:1576-1701, fixed-function raster, depth test GREATER on the reverse-Z buffer), in its three submission
 // modes:
-//   cluster submit  vkCmdDrawMeshTasksIndirectEXT(ccb, 4) -> meshlet.mesh.glsl:89-206 over cib       raster_clusters_kernel<false>
+//   cluster submit  vkCmdDrawMeshTasksIndirectEXT(ccb, 4) -> meshlet.mesh.glsl:89-206 over cib       raster_clusters_kernel<false, *>
 //   task shading    vkCmdDrawMeshTasksIndirectEXT(dccb, 4) -> meshlet.task EmitMeshTasksEXT(n) ->
-//                   meshlet.mesh.glsl (TASK = true) over the task payloads                            raster_clusters_kernel<true>
+//                   meshlet.mesh.glsl (TASK = true) over the task payloads                            raster_clusters_kernel<true, *>
+//   (second parameter: the mesh shader's per-triangle cull stage, MESH_CULL = 1, nvc_set_mesh_cull)
 //   indexed draws   vkCmdDrawIndexedIndirectCount(dcb + 4, dccb, 0, maxDrawCount, 24) -> mesh.vert    raster_indexed_kernel
 // Cluster modes: one warp per cluster; the lanes transform the <= 64 vertices exactly as the mesh shader does (strict IEEE, GLSL
 // operation order) into shared memory, then each lane rasterises its share of the <= 96 triangles.  Indexed mode: one warp per
@@ -2017,6 +2018,30 @@ __device__ __forceinline__ void raster_triangle(const float4 (&pc)[3], float* de
 		}
 }
 
+// The per-triangle cull stage of meshlet.mesh.glsl:175-195 (compiled in with MESH_CULL = 1): true when the mesh shader marks the
+// triangle gl_CullPrimitiveEXT.  p = (clip.xy / clip.w * 0.5 + 0.5) * screen is the float fx / fy of raster_triangle (meshlet.mesh.glsl:150
+// keeps it in vertexClip); back faces and zero area: eb.x * ec.y <= eb.y * ec.x with two rounded products; small primitives: the
+// bounding box rounds to one column or one row, sbprec = 1/256, `round` = roundf (halfway away from zero, the rule the host shim
+// uses); all of it only when every corner has w > 0.  min / max are IEEE minNum / maxNum (a NaN corner drops out of the box, as in the
+// shim); every comparison with a NaN operand is false, so a NaN w is never culled and reaches raster_triangle, which drops it.
+__device__ __forceinline__ bool mesh_cull_triangle(const float4 (&pc)[3], float sw, float sh)
+{
+	float px[3], py[3];
+#pragma unroll
+	for (int c = 0; c < 3; ++c)
+	{
+		px[c] = __fmul_rn(__fadd_rn(__fmul_rn(__fdiv_rn(pc[c].x, pc[c].w), 0.5f), 0.5f), sw);
+		py[c] = __fmul_rn(__fadd_rn(__fmul_rn(__fdiv_rn(pc[c].y, pc[c].w), 0.5f), 0.5f), sh);
+	}
+	const float ebx = __fsub_rn(px[1], px[0]), eby = __fsub_rn(py[1], py[0]), ecx = __fsub_rn(px[2], px[0]), ecy = __fsub_rn(py[2], py[0]);
+	bool culled = __fmul_rn(ebx, ecy) <= __fmul_rn(eby, ecx);
+	const float bminx = fminf(px[0], fminf(px[1], px[2])), bmaxx = fmaxf(px[0], fmaxf(px[1], px[2]));
+	const float bminy = fminf(py[0], fminf(py[1], py[2])), bmaxy = fmaxf(py[0], fmaxf(py[1], py[2]));
+	const float sbprec = 1.0f / 256.0f;
+	culled = culled || roundf(__fsub_rn(bminx, sbprec)) == roundf(bmaxx) || roundf(bminy) == roundf(__fadd_rn(bmaxy, sbprec));
+	return culled && pc[0].w > 0.0f && pc[1].w > 0.0f && pc[2].w > 0.0f;
+}
+
 // warp-reduces the four per-lane counters and adds them to stats4 (nullptr: not wanted)
 __device__ __forceinline__ void flush_stats4(uint32_t* stats4, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3)
 {
@@ -2067,12 +2092,16 @@ struct RasterParams
 	// clusters / commands drawn, triangles rasterised, clusters / commands rejected (data out of range), cluster modes: depth
 	// updates issued, indexed draws: triangles rejected (vertex index out of range)
 	uint32_t* stats4;
+	// MeshCull instantiations: triangles tested and culled by the mesh-cull stage, added to these two context-owned counters
+	unsigned long long* mesh_cull2;
 };
 
 // Task = false: work item w is slot x + y * 256 + z * 16 of the (16, Y, 16) dispatch in ccb, reading cib (meshlet.mesh.glsl:94).
 // Task = true: work item w is mesh workgroup i = w % 64 of task command c = w / 64 of the (X, 64, 1) dispatch in dccb; it exists when
 // i < min(emit_counts[c], 64) and reads payloads[c].clusterIndices[i].  Everything after the cluster index is the same code.
-template <bool Task>
+// MeshCull = true: a triangle that passes the index checks is first given the mesh-cull decision (mesh_cull_triangle) and only
+// sampled when not culled; tested / culled triangles are added to p.mesh_cull2.
+template <bool Task, bool MeshCull>
 __global__ void __launch_bounds__(kRasterWarps * 32) raster_clusters_kernel(const RasterParams p)
 {
 	__shared__ float4 s_clip[kRasterWarps][64];
@@ -2087,7 +2116,7 @@ __global__ void __launch_bounds__(kRasterWarps * 32) raster_clusters_kernel(cons
 		items = gx * p.cluster_count4[2] * gz;
 	}
 	float4* clip = s_clip[warp];
-	uint32_t drawn = 0, tris = 0, rejected = 0, writes = 0;
+	uint32_t drawn = 0, tris = 0, rejected = 0, writes = 0, tested = 0, culled = 0;
 	const double fw = double(p.width), fh = double(p.height);
 
 	for (uint32_t w = blockIdx.x * kRasterWarps + warp; w < items; w += gridDim.x * kRasterWarps)
@@ -2155,11 +2184,34 @@ __global__ void __launch_bounds__(kRasterWarps * 32) raster_clusters_kernel(cons
 			if (ia >= vertexCount || ib >= vertexCount || ic >= vertexCount)
 				continue;
 			const float4 pc[3] = { clip[ia], clip[ib], clip[ic] };
+			if (MeshCull)
+			{
+				++tested;
+				if (mesh_cull_triangle(pc, float(p.width), float(p.height)))
+				{
+					++culled;
+					continue; // gl_CullPrimitiveEXT
+				}
+			}
 			raster_triangle(pc, p.depth, p.width, p.height, fw, fh, tris, writes);
 		}
 		__syncwarp(); // the next cluster reuses clip[]
 	}
 	flush_stats4(p.stats4, drawn, tris, rejected, writes);
+	if (MeshCull)
+	{
+#pragma unroll
+		for (int o = 16; o >= 1; o >>= 1)
+		{
+			tested += __shfl_xor_sync(0xffffffffu, tested, o);
+			culled += __shfl_xor_sync(0xffffffffu, culled, o);
+		}
+		if (lane == 0 && tested)
+		{
+			atomicAdd(p.mesh_cull2 + 0, (unsigned long long)tested);
+			atomicAdd(p.mesh_cull2 + 1, (unsigned long long)culled);
+		}
+	}
 }
 
 // Commands i < min(command_count4[0], max_draw_count) of dcb, each split into kIndexedSlices equal runs of its indexCount / 3
@@ -2252,7 +2304,7 @@ cudaError_t launch_raster(void (*kernel)(RasterParams), const RasterParams& p, u
 
 cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pass, const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands,
     const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width,
-    uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream)
+    uint32_t height, uint32_t* stats4, unsigned long long* mesh_cull2, uint32_t blocks, cudaStream_t stream)
 {
 	RasterParams p = raster_params(projection16, pass, draws, vertices, vertex_count, depth, width, height, stats4);
 	p.cluster_indices = cluster_indices;
@@ -2261,12 +2313,13 @@ cudaError_t launch_raster_depth(const float* projection16, const NvcCullData& pa
 	p.meshlets = meshlets;
 	p.meshletdata = meshletdata;
 	p.meshletdata_words = meshletdata_words;
-	return launch_raster(raster_clusters_kernel<false>, p, blocks, stream);
+	p.mesh_cull2 = mesh_cull2;
+	return launch_raster(mesh_cull2 ? raster_clusters_kernel<false, true> : raster_clusters_kernel<false, false>, p, blocks, stream);
 }
 
 cudaError_t launch_raster_depth_tasks(const float* projection16, const NvcCullData& pass, const NvcMeshTaskPayload* payloads, const uint32_t* emit_counts, const uint32_t* command_count4,
     const NvcMeshTaskCommand* task_commands, const NvcMeshDraw* draws, const NvcMeshlet* meshlets, const uint32_t* meshletdata, uint32_t meshletdata_words, const NvcVertex* vertices,
-    uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4, uint32_t blocks, cudaStream_t stream)
+    uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4, unsigned long long* mesh_cull2, uint32_t blocks, cudaStream_t stream)
 {
 	RasterParams p = raster_params(projection16, pass, draws, vertices, vertex_count, depth, width, height, stats4);
 	p.payloads = payloads;
@@ -2276,7 +2329,8 @@ cudaError_t launch_raster_depth_tasks(const float* projection16, const NvcCullDa
 	p.meshlets = meshlets;
 	p.meshletdata = meshletdata;
 	p.meshletdata_words = meshletdata_words;
-	return launch_raster(raster_clusters_kernel<true>, p, blocks, stream);
+	p.mesh_cull2 = mesh_cull2;
+	return launch_raster(mesh_cull2 ? raster_clusters_kernel<true, true> : raster_clusters_kernel<true, false>, p, blocks, stream);
 }
 
 cudaError_t launch_raster_depth_indexed(const float* projection16, const NvcCullData& pass, const NvcMeshDrawCommand* draw_commands, const uint32_t* command_count4, uint32_t max_draw_count,

@@ -157,6 +157,18 @@ class VisibilityPath:
         assert depth.dtype == torch.float32 and depth.is_contiguous() and depth.numel() == self.depth_width * self.depth_height
         check(self.lib.nvc_depth_pyramid(self.ctx, self._stream(), _ptr(depth), self.depth_width, self.depth_height, ctypes.byref(self.hiz)), self.ctx, "nvc_depth_pyramid")
 
+    def set_mesh_cull(self, enabled):
+        """The mesh shader's per-triangle cull stage (meshlet.mesh.glsl with MESH_CULL = 1) in raster_depth and raster_depth_tasks
+        calls made after this one: back-facing, zero-area and small triangles are not sampled.  Off by default, as in the reference;
+        raster_depth_indexed is not affected."""
+        check(self.lib.nvc_set_mesh_cull(self.ctx, int(bool(enabled))), self.ctx, "nvc_set_mesh_cull")
+
+    def mesh_cull_stats(self, reset=False):
+        """(triangles tested, triangles culled) by the mesh-cull stage since the last reset (synchronises the device)."""
+        out = (ctypes.c_uint64 * 2)()
+        check(self.lib.nvc_mesh_cull_stats(self.ctx, out, int(bool(reset))), self.ctx, "nvc_mesh_cull_stats")
+        return int(out[0]), int(out[1])
+
     def raster_depth(self, cull_data, projection16, vertices, meshletdata, depth, stats=None):
         """Depth-only consumer of this path's cib / ccb / dcb on the device (nvc_raster_depth): what the reference's mesh stage +
         rasteriser do to the depth target between the cull passes.  vertices: uint8 device tensor of 16-byte Vertex records;

@@ -9,7 +9,10 @@
 Every pass is timed with CUDA events over --steps frames after --warmup frames; one JSON line per mode with the median and minimum of
 every pass, the frame time, the triangles rasterised, the visible draws / clusters and the card (name, power limit, max SM clock from
 nvidia-smi).  The last frame is run twice from the same visibility state and must give the same depth bits.  Needs a CUDA device;
-writes nothing."""
+writes nothing.
+
+--mesh-cull: the cluster and task modes only, each run with the mesh shader's per-triangle cull stage (nvc_set_mesh_cull) off and on,
+alternating, --rounds times in one process; every line then also carries "mesh_cull" and the triangles the stage culled per pass."""
 import argparse
 import json
 import os
@@ -35,7 +38,7 @@ def card():
     return {"device": name or torch.cuda.get_device_name(0), "power_limit": power, "sm_clock_max": clock}
 
 
-def run_mode(mode, s, geometry, args):
+def run_mode(mode, s, geometry, args, mesh_cull=None):
     dev = torch.device("cuda:0")
     mesh_shading = mode != "indexed"
     kw = {}
@@ -45,6 +48,8 @@ def run_mode(mode, s, geometry, args):
         kw["task_wglimit"] = int((per_draw.sum() + 63) // 64 * 64)
     path = VisibilityPath(s.meshes, s.meshlets, s.draws, *s.screen, mesh_shading=mesh_shading, **kw)
     path.set_visibility_bits(s.visibility_bits)
+    if mesh_cull is not None:
+        path.set_mesh_cull(mesh_cull)
     cd = s.cull_data(**({} if mesh_shading else dict(mesh_shading=False, cluster_occlusion=False)))
     proj = host.projection(s.camera, *s.screen)
     vb = torch.from_numpy(np.ascontiguousarray(geometry["vertices"])).to(dev)
@@ -86,6 +91,8 @@ def run_mode(mode, s, geometry, args):
         mark(2)
         depth.zero_()
         raster(0)
+        if probe and mesh_cull is not None:
+            counts["culled_early"] = path.mesh_cull_stats(reset=True)[1]
         mark(3)
         path.pyramid(depth)
         mark(4)
@@ -97,6 +104,8 @@ def run_mode(mode, s, geometry, args):
             counts["clusters_late"] = int(path.ccb[0].item()) if mode == "cluster" else int(emit[: int(path.dccb[1].item()) * 64].clamp(max=64).sum().item()) if mode == "tasks" else None
         mark(6)
         raster(1)
+        if probe and mesh_cull is not None:
+            counts["culled_late"] = path.mesh_cull_stats(reset=True)[1]
         mark(7)
 
     for _ in range(max(3, args.warmup)):
@@ -110,6 +119,8 @@ def run_mode(mode, s, geometry, args):
 
     # determinism: the last frame again from the same visibility state, twice
     dvb, mvb = path.dvb.clone(), path.mvb.clone()
+    if mesh_cull is not None:
+        path.mesh_cull_stats(reset=True)
     frame(probe=True)
     torch.cuda.synchronize()
     first = depth.clone()
@@ -138,6 +149,9 @@ def run_mode(mode, s, geometry, args):
         "clusters": None if mode == "indexed" else {"early": counts["clusters_early"], "late": counts["clusters_late"]},
         "rejected": {"early": int(st[0][2]), "late": int(st[1][2])},
     }
+    if mesh_cull is not None:
+        out["mesh_cull"] = bool(mesh_cull)
+        out["triangles_culled"] = {"early": counts["culled_early"], "late": counts["culled_late"]}
     out.update(card())
     path.close()
     return out
@@ -150,6 +164,8 @@ def main():
     ap.add_argument("--draws", type=int, default=10000)
     ap.add_argument("--depth", type=int, default=4096, help="depth target size (square)")
     ap.add_argument("--modes", default="cluster,tasks,indexed")
+    ap.add_argument("--mesh-cull", action="store_true", help="cluster / task modes with the mesh-cull stage off and on, alternating")
+    ap.add_argument("--rounds", type=int, default=3, help="off / on pairs per mode with --mesh-cull")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("raster_modes_bench.py needs a CUDA device")
@@ -160,6 +176,14 @@ def main():
     cache = scene_cache.SceneCache(os.path.join(golden, "kitten.z.cache"))
     if not np.array_equal(cache.section("meshes"), s.meshes):
         sys.exit("kitten.z.cache does not hold the meshes of kitten.nvcg")
+    if args.mesh_cull:
+        modes = [m for m in args.modes.split(",") if m != "indexed"]  # mesh.vert has no per-triangle stage
+        geometry = {"vertices": s.vertices, "indices": cache.section("indices")}
+        for r in range(args.rounds):
+            for mode in modes:
+                for on in ((False, True) if r % 2 == 0 else (True, False)):
+                    print(json.dumps(run_mode(mode, s, geometry, args, mesh_cull=on)), flush=True)
+        return
     for mode in args.modes.split(","):
         geometry = {"vertices": s.vertices if mode != "indexed" else cache.section("vertices"), "indices": cache.section("indices")}
         print(json.dumps(run_mode(mode, s, geometry, args)), flush=True)
