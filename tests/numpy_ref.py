@@ -184,7 +184,9 @@ def drawcull_decisions(cd, late, draws, meshes, dvb, levels=None):
     emit = reached & visible & cond
     lod = np.zeros(n, dtype=np.uint32)
     if cd["lodEnabled"] == 1:
-        dist = np.maximum(length3(center) - radius, F(0.0))
+        # max(NaN, 0) = 0: IEEE maxNum, as GPU hardware, the kernels and the oracle take it (a NaN draw position selects by threshold 0)
+        with np.errstate(invalid="ignore"):
+            dist = np.fmax(length3(center) - radius, F(0.0))
         thr = dist * F(cd["lodTarget"]) / d["scale"]
         for i in range(1, layout_max_lods(meshes)):
             sel = (i < mesh["lodCount"]) & (mesh["lods"]["error"][:, i] < thr)
