@@ -591,6 +591,22 @@ NVC_API int nvc_set_mesh_cull(NvcContext* ctx, int enabled);
  * cumulative since the last call with reset != 0. */
 NVC_API int nvc_mesh_cull_stats(NvcContext* ctx, uint64_t* out_tested_culled2, int reset);
 
+/* The reference's TASK_CULL switch (config.h:8, "meshlet frustum, occlusion and backface culling in the task shader"; the
+ * reference default and the default here are 1).  With enabled = 0, calls enqueued after this one behave as a TASK_CULL 0 build:
+ *   nvc_drawcull     the late pass emits only draws that were not visible last frame, plus post-pass draws
+ *                    (drawcull.comp.glsl:104 without its clusterOcclusionEnabled term), in both task and draw modes;
+ *   nvc_clustercull  every lane mgi < min(taskCount, 64) of every command c < command_count4[1] * 64 appends c | (mgi << 24)
+ *                    (clustercull.comp.glsl:140-147), with the usual cluster_limit overflow rule and the clustersubmit epilogue;
+ *   nvc_taskcull     payloads[c].clusterIndices[i] = c | (i << 24) for all 64 entries and emit_counts[c] = taskCount as stored,
+ *                    not clamped to 64 (meshlet.task.glsl:144-148), padding commands included.
+ * The cluster and task passes then test no meshlet: they read only task_commands and command_count4; draws, meshlets, the Hi-Z
+ * and meshlet_visibility are not read, and meshlet_visibility is not written.  Argument validation is unchanged, so callers pass
+ * the same buffers either way.  Turning the switch back on mid-sequence makes the cluster passes read visibility bits nobody
+ * maintained while it was off (the reference has no runtime switch, so no reference behaviour covers that).  The setting is read
+ * when a call is enqueued: a captured graph keeps the value that was current at capture time.  The multi-GPU exchange
+ * (nvc_gather_*) is not covered with the switch off. */
+NVC_API int nvc_set_task_cull(NvcContext* ctx, int enabled);
+
 /* Recomputes center / radius / cone_axis / cone_cutoff of meshlets[0..meshlet_count) from geometry, bit-identical to
  * what the reference's cooker stores (scene.cpp:69-80 appendMeshlet -> meshopt_computeMeshletBounds,
  * meshletutils.cpp:133-272,314-339): one thread per meshlet reads its references and triangles from

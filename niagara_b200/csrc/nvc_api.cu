@@ -373,6 +373,10 @@ NVC_API int nvc_drawcull(NvcContext* ctx, void* stream, const NvcCullData* cull,
 	nvc::DrawCullParams p;
 	memset(&p, 0, sizeof(p));
 	p.cull = *cull;
+	// TASK_CULL = 0: drawcull.comp.glsl:104 loses its (clusterOcclusionEnabled == 1 && TASK_CULL == 1) term; the kernel reads the
+	// field only there
+	if (!ctx->task_cull)
+		p.cull.clusterOcclusionEnabled = 0;
 	p.draws = draws;
 	p.meshes = meshes;
 	if (ctx->mesh_heads && ctx->prepared_meshes == meshes)
@@ -455,6 +459,11 @@ NVC_API int nvc_clustercull(NvcContext* ctx, void* stream, const NvcCullData* cu
 		return s;
 	p.cluster_indices = cluster_indices;
 	p.cluster_count4 = cluster_count4;
+	if (!ctx->task_cull)
+	{
+		cudaError_t e = nvc::launch_clustercull_passthrough(p, uint32_t(ctx->sm_count) * 8u, static_cast<cudaStream_t>(stream));
+		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_clustercull");
+	}
 
 	bool staged = false;
 	if (late && cull->clusterOcclusionEnabled == 1 && hiz)
@@ -499,6 +508,11 @@ NVC_API int nvc_taskcull(NvcContext* ctx, void* stream, const NvcCullData* cull,
 	int s = fill_cluster_params(ctx, cull, late, task_commands, command_count4, draws, meshlets, meshlet_visibility, hiz, p);
 	if (s != NVC_OK)
 		return s;
+	if (!ctx->task_cull)
+	{
+		cudaError_t e = nvc::launch_taskcull_passthrough(task_commands, command_count4, payloads, emit_counts, uint32_t(ctx->sm_count) * 8u, static_cast<cudaStream_t>(stream));
+		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_taskcull");
+	}
 	uint32_t blocks = uint32_t(ctx->sm_count) * 4u;
 	if (ctx->cluster_filter)
 	{
@@ -523,6 +537,14 @@ NVC_API int nvc_decode_clusters(NvcContext* ctx, void* stream, const uint32_t* c
 		return NVC_ERROR_INVALID_ARGUMENT;
 	cudaError_t e = nvc::launch_decode_clusters(cluster_indices, cluster_count4, task_commands, meshlets, records, stats4, uint32_t(ctx->sm_count) * 8u, static_cast<cudaStream_t>(stream));
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_decode_clusters");
+}
+
+NVC_API int nvc_set_task_cull(NvcContext* ctx, int enabled)
+{
+	if (!ctx)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	ctx->task_cull = enabled != 0;
+	return NVC_OK;
 }
 
 // the mesh-cull counters when the stage is on (read when the call is enqueued), nullptr when it is off

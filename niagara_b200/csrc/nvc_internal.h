@@ -22,6 +22,7 @@ struct NvcContext
 	bool draw_filter = false;   // env NVC_DRAW_FILTER=1: filtered occlusion stage of the late drawcull (off by default: the pass is not issue bound)
 	bool cluster_filter = true; // nvc_set_cluster_filter / env NVC_CLUSTER_FILTER: filtered cluster kernel (default) or the exact one
 	bool mesh_cull = false;     // nvc_set_mesh_cull: the mesh shader's per-triangle cull stage (MESH_CULL) in the cluster-mode depth producers
+	bool task_cull = true;      // nvc_set_task_cull: meshlet culling in the cluster / task passes (TASK_CULL); off = pass-through
 	uint32_t hiz_stage_budget = 0; // texels (24 KB) of coarse Hi-Z mips staged per CTA; 0 = off (env NVC_HIZ_STAGE_TEXELS)
 	NvcLimits limits = { NVC_TASK_WGLIMIT, NVC_CLUSTER_LIMIT };
 	nvc::Scratch* scratch = nullptr;
@@ -199,6 +200,10 @@ struct PyramidParams
 cudaError_t launch_drawcull(const DrawCullParams& p, bool late, bool task, cudaStream_t stream);
 cudaError_t launch_clustercull(const ClusterParams& p, bool late, uint32_t blocks, cudaStream_t stream);
 cudaError_t launch_taskcull(const ClusterParams& p, bool late, NvcMeshTaskPayload* payloads, uint32_t* emit_counts, uint32_t blocks, cudaStream_t stream);
+// TASK_CULL = 0: the cluster / task passes without meshlet tests (read only the task commands and their count)
+cudaError_t launch_clustercull_passthrough(const ClusterParams& p, uint32_t blocks, cudaStream_t stream);
+cudaError_t launch_taskcull_passthrough(const NvcMeshTaskCommand* task_commands, const uint32_t* command_count4, NvcMeshTaskPayload* payloads, uint32_t* emit_counts, uint32_t blocks,
+    cudaStream_t stream);
 cudaError_t launch_pyramid(const PyramidParams& p, cudaStream_t stream);
 cudaError_t launch_footprint(const HiZDesc& hiz, float* fp, uint32_t total, cudaStream_t stream);
 cudaError_t launch_decode_clusters(const uint32_t* cluster_indices, const uint32_t* cluster_count4, const NvcMeshTaskCommand* task_commands, const NvcMeshlet* meshlets, NvcClusterRecord* records, uint32_t* stats4, uint32_t blocks, cudaStream_t stream);

@@ -1607,6 +1607,134 @@ __global__ void __launch_bounds__(kClusterBlock) taskcull_kernel(const ClusterPa
 }
 
 // ------------------------------------------------------------------------------------------------------
+// TASK_CULL = 0 (nvc_set_task_cull(ctx, 0)): the cluster and task passes without meshlet tests.  Only the task commands are
+// read; draws, meshlets, meshlet visibility and the Hi-Z are not touched.
+// ------------------------------------------------------------------------------------------------------
+
+constexpr uint32_t kPassBlock = 256; // task commands per tile (one thread each)
+
+// clustercull.comp.glsl:140-147 + clustersubmit.comp.glsl:25-45: every lane mgi < taskCount of command c < command_count4[1] * 64
+// appends c | (mgi << 24) (mgi < 64: the workgroup has 64 lanes).  Per tile of 256 commands: one thread loads a command's
+// taskCount, a block-wide scan gives each command its offset, ONE atomicAdd on the cluster counter reserves the tile's contiguous
+// range, and each warp writes whole commands with consecutive stores.  The counter counts past cluster_limit; stores at or above
+// it are dropped.  The last CTA runs the clustersubmit epilogue and leaves the scratch counters zeroed.
+__global__ void __launch_bounds__(kPassBlock) clustercull_passthrough_kernel(const ClusterParams p)
+{
+	__shared__ uint32_t s_count[kPassBlock], s_offset[kPassBlock];
+	__shared__ uint32_t s_warp_total[kPassBlock / 32];
+	__shared__ uint32_t s_base, s_is_last;
+
+	const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+	const uint32_t ncmd = p.command_count4[1] * 64u;
+	for (uint32_t tile = blockIdx.x * kPassBlock; tile < ncmd; tile += gridDim.x * kPassBlock)
+	{
+		const uint32_t cid = tile + tid;
+		const uint32_t count = cid < ncmd ? min(__ldg(reinterpret_cast<const uint32_t*>(p.task_commands + cid) + 2), NVC_TASK_WGSIZE) : 0u;
+		uint32_t incl = count;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1)
+		{
+			const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o);
+			if (lane >= uint32_t(o))
+				incl += n;
+		}
+		if (lane == 31)
+			s_warp_total[warp] = incl;
+		__syncthreads();
+		if (warp == 0)
+		{
+			const uint32_t t = lane < kPassBlock / 32 ? s_warp_total[lane] : 0u;
+			uint32_t ti = t;
+#pragma unroll
+			for (int o = 1; o < int(kPassBlock / 32); o <<= 1)
+			{
+				const uint32_t n = __shfl_up_sync(0xffffffffu, ti, o);
+				if (lane >= uint32_t(o))
+					ti += n;
+			}
+			if (lane < kPassBlock / 32)
+				s_warp_total[lane] = ti - t; // exclusive warp offsets
+			const uint32_t total = __shfl_sync(0xffffffffu, ti, kPassBlock / 32 - 1);
+			if (lane == 0)
+				s_base = total ? atomicAdd(&p.scratch->cluster_counter, total) : 0u; // :143, aggregated
+		}
+		__syncthreads();
+		s_count[tid] = count;
+		s_offset[tid] = s_warp_total[warp] + incl - count;
+		__syncthreads();
+		const uint32_t base = s_base;
+		for (uint32_t c = warp; c < kPassBlock; c += kPassBlock / 32)
+		{
+			const uint32_t n = s_count[c], first = base + s_offset[c];
+			for (uint32_t mgi = lane; mgi < n; mgi += 32)
+				if (first + mgi < p.cluster_limit) // :145
+					p.cluster_indices[first + mgi] = (tile + c) | (mgi << 24);
+		}
+		__syncthreads(); // s_count / s_offset / s_warp_total are reused by the next tile
+	}
+
+	// ---- last-block epilogue: clustersubmit.comp.glsl:25-45 (as in clustercull_kernel) ----
+	__threadfence();
+	__syncthreads();
+	if (tid == 0)
+		s_is_last = atomicAdd(&p.scratch->cluster_done, 1u) == gridDim.x - 1;
+	__syncthreads();
+	if (!s_is_last)
+		return;
+	__threadfence();
+
+	const uint32_t clusterCount = *reinterpret_cast<volatile uint32_t*>(&p.scratch->cluster_counter);
+	const uint32_t count = min(clusterCount, p.cluster_limit);
+	if (tid == 0)
+	{
+		p.cluster_count4[0] = clusterCount;
+		p.cluster_count4[1] = NVC_CLUSTER_TILE;
+		p.cluster_count4[2] = min((count + 255) / 256, NVC_MAX_DISPATCH_GROUPS);
+		p.cluster_count4[3] = 256 / NVC_CLUSTER_TILE;
+	}
+	const uint32_t boundary = (count + 255) & ~255u;
+	if (count + tid < boundary) // blockDim == 256 == clustersubmit's local_size_x
+		p.cluster_indices[count + tid] = ~0u;
+	__syncthreads();
+	if (tid == 0)
+	{
+		p.scratch->cluster_counter = 0;
+		p.scratch->cluster_done = 0;
+		p.scratch->cluster_batch = 0;
+	}
+}
+
+// meshlet.task.glsl:144-148: for every command c < command_count4[1] * 64, all 64 lanes write payload.clusterIndices[lane] =
+// c | (lane << 24), taskCount or not, and the shader emits taskCount mesh workgroups, as read (not clamped to 64).  A pure
+// streaming write: 16 bytes of payload per thread step (4 bytes when payloads is not 16-byte aligned), emit_counts[c] from the
+// command's taskCount.
+__global__ void __launch_bounds__(kPassBlock) taskcull_passthrough_kernel(const NvcMeshTaskCommand* __restrict__ task_commands, const uint32_t* __restrict__ command_count4,
+    NvcMeshTaskPayload* __restrict__ payloads, uint32_t* __restrict__ emit_counts)
+{
+	const uint32_t ncmd = __ldg(command_count4 + 1) * 64u;
+	const uint32_t stride = gridDim.x * kPassBlock;
+	const uint32_t first = blockIdx.x * kPassBlock + threadIdx.x;
+	for (uint32_t c = first; c < ncmd; c += stride)
+		emit_counts[c] = __ldg(reinterpret_cast<const uint32_t*>(task_commands + c) + 2);
+	uint32_t* const words = reinterpret_cast<uint32_t*>(payloads);
+	if ((reinterpret_cast<uintptr_t>(payloads) & 15u) == 0)
+	{
+		const uint32_t nvec = ncmd * (NVC_TASK_WGSIZE / 4);
+		for (uint32_t v = first; v < nvec; v += stride)
+		{
+			const uint32_t c = v / (NVC_TASK_WGSIZE / 4), lane = (v % (NVC_TASK_WGSIZE / 4)) * 4u;
+			reinterpret_cast<uint4*>(words)[v] = make_uint4(c | (lane << 24), c | ((lane + 1u) << 24), c | ((lane + 2u) << 24), c | ((lane + 3u) << 24));
+		}
+	}
+	else
+	{
+		const uint32_t nword = ncmd * NVC_TASK_WGSIZE;
+		for (uint32_t w = first; w < nword; w += stride)
+			words[w] = (w / NVC_TASK_WGSIZE) | ((w % NVC_TASK_WGSIZE) << 24);
+	}
+}
+
+// ------------------------------------------------------------------------------------------------------
 // depth pyramid: all mips in ONE launch.
 // Each CTA owns a 64x64 tile of mip 0 (128x128 depth texels when the ratio is exactly 2:1), reduces it through
 // mips 0..6 in shared memory, writing every level; the last CTA to finish (global ticket) reduces the remaining
@@ -2680,6 +2808,19 @@ cudaError_t launch_taskcull(const ClusterParams& p, bool late, NvcMeshTaskPayloa
 		taskcull_kernel<true><<<blocks, kClusterBlock, 0, stream>>>(p, payloads, emit_counts);
 	else
 		taskcull_kernel<false><<<blocks, kClusterBlock, 0, stream>>>(p, payloads, emit_counts);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_clustercull_passthrough(const ClusterParams& p, uint32_t blocks, cudaStream_t stream)
+{
+	clustercull_passthrough_kernel<<<blocks, kPassBlock, 0, stream>>>(p);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_taskcull_passthrough(const NvcMeshTaskCommand* task_commands, const uint32_t* command_count4, NvcMeshTaskPayload* payloads, uint32_t* emit_counts, uint32_t blocks,
+    cudaStream_t stream)
+{
+	taskcull_passthrough_kernel<<<blocks, kPassBlock, 0, stream>>>(task_commands, command_count4, payloads, emit_counts);
 	return cudaGetLastError();
 }
 

@@ -42,6 +42,7 @@ SIGNATURES = [
     ("nvc_filter_stats", ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_uint64), ctypes.c_int]),
     ("nvc_set_mesh_cull", ctypes.c_int, [c_void_p, ctypes.c_int]),
     ("nvc_mesh_cull_stats", ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_uint64), ctypes.c_int]),
+    ("nvc_set_task_cull", ctypes.c_int, [c_void_p, ctypes.c_int]),
     ("nvc_previous_pow2", ctypes.c_uint32, [ctypes.c_uint32]),
     ("nvc_image_mip_levels", ctypes.c_uint32, [ctypes.c_uint32, ctypes.c_uint32]),
     ("nvc_hiz_layout", ctypes.c_int, [ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(HiZ)]),

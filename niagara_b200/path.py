@@ -163,6 +163,12 @@ class VisibilityPath:
         raster_depth_indexed is not affected."""
         check(self.lib.nvc_set_mesh_cull(self.ctx, int(bool(enabled))), self.ctx, "nvc_set_mesh_cull")
 
+    def set_task_cull(self, enabled):
+        """The reference's TASK_CULL switch for cull, render_clusters and task_shading calls made after this one.
+        Off: the late drawcull emits only draws not visible last frame (plus post-pass draws), and the cluster and task passes pass
+        every meshlet of every command through without a test, leaving mvb untouched.  On by default, as in the reference."""
+        check(self.lib.nvc_set_task_cull(self.ctx, int(bool(enabled))), self.ctx, "nvc_set_task_cull")
+
     def mesh_cull_stats(self, reset=False):
         """(triangles tested, triangles culled) by the mesh-cull stage since the last reset (synchronises the device)."""
         out = (ctypes.c_uint64 * 2)()

@@ -12,7 +12,12 @@ nvidia-smi).  The last frame is run twice from the same visibility state and mus
 writes nothing.
 
 --mesh-cull: the cluster and task modes only, each run with the mesh shader's per-triangle cull stage (nvc_set_mesh_cull) off and on,
-alternating, --rounds times in one process; every line then also carries "mesh_cull" and the triangles the stage culled per pass."""
+alternating, --rounds times in one process; every line then also carries "mesh_cull" and the triangles the stage culled per pass.
+
+--task-cull: the cluster and task modes only, each run with the reference's TASK_CULL switch (nvc_set_task_cull) off and on,
+alternating, --rounds times in one process; every line then also carries "task_cull".  After them, one "passthrough" line per pass
+times the TASK_CULL 0 cluster and task passes alone on the C4 scene (1 M draws, early pass) and gives the bytes they must move
+over kernel time as a share of the H100 SXM's 3.35 TB/s."""
 import argparse
 import json
 import os
@@ -38,7 +43,7 @@ def card():
     return {"device": name or torch.cuda.get_device_name(0), "power_limit": power, "sm_clock_max": clock}
 
 
-def run_mode(mode, s, geometry, args, mesh_cull=None):
+def run_mode(mode, s, geometry, args, mesh_cull=None, task_cull=None):
     dev = torch.device("cuda:0")
     mesh_shading = mode != "indexed"
     kw = {}
@@ -50,6 +55,8 @@ def run_mode(mode, s, geometry, args, mesh_cull=None):
     path.set_visibility_bits(s.visibility_bits)
     if mesh_cull is not None:
         path.set_mesh_cull(mesh_cull)
+    if task_cull is not None:
+        path.set_task_cull(task_cull)
     cd = s.cull_data(**({} if mesh_shading else dict(mesh_shading=False, cluster_occlusion=False)))
     proj = host.projection(s.camera, *s.screen)
     vb = torch.from_numpy(np.ascontiguousarray(geometry["vertices"])).to(dev)
@@ -152,7 +159,46 @@ def run_mode(mode, s, geometry, args, mesh_cull=None):
     if mesh_cull is not None:
         out["mesh_cull"] = bool(mesh_cull)
         out["triangles_culled"] = {"early": counts["culled_early"], "late": counts["culled_late"]}
+    if task_cull is not None:
+        out["task_cull"] = bool(task_cull)
     out.update(card())
+    path.close()
+    return out
+
+
+def passthrough_c4(args):
+    """the TASK_CULL 0 cluster and task passes alone on the C4 scene's early commands: CUDA events around --steps launches each"""
+    s = scenes.config4_scene()
+    path = VisibilityPath(s.meshes, s.meshlets, s.draws, *s.screen)
+    path.set_visibility_bits(s.visibility_bits)
+    path.set_task_cull(False)
+    path.dvb.fill_(1)
+    cd = s.cull_data()
+    path.cull(cd, late=False)
+    torch.cuda.synchronize()
+    ncmd = int(path.dccb[1].item()) * 64
+    payloads = torch.empty((ncmd, 64), dtype=torch.int32, device="cuda:0")
+    emit = torch.empty(ncmd, dtype=torch.int32, device="cuda:0")
+    runs = {"clusters": lambda: path.render_clusters(cd, False), "tasks": lambda: path.task_shading(cd, False, payloads, emit)}
+    out = []
+    for name, run in runs.items():
+        for _ in range(max(3, args.warmup)):
+            run()
+        torch.cuda.synchronize()
+        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
+        for a, b in evs:
+            a.record()
+            run()
+            b.record()
+        torch.cuda.synchronize()
+        ms = np.array([a.elapsed_time(b) for a, b in evs])
+        clusters = int(path.ccb[0].item())
+        # every 32-byte sector of the 20-byte command records holds a taskCount that is read; output as written
+        moved = ncmd * 20 + (clusters + 255) // 256 * 256 * 4 if name == "clusters" else ncmd * 20 + ncmd * (256 + 4)
+        med = float(np.median(ms))
+        out.append({"passthrough": name, "workload": "C4: %d draws, early pass, %d task commands" % (len(s.draws), ncmd), "steps": args.steps,
+                    "kernel_ms": {"median": med, "min": float(ms.min())}, "clusters": clusters if name == "clusters" else None, "bytes": moved,
+                    "share_of_3.35TBps": moved / (med * 1e-3) / 3.35e12})
     path.close()
     return out
 
@@ -165,7 +211,8 @@ def main():
     ap.add_argument("--depth", type=int, default=4096, help="depth target size (square)")
     ap.add_argument("--modes", default="cluster,tasks,indexed")
     ap.add_argument("--mesh-cull", action="store_true", help="cluster / task modes with the mesh-cull stage off and on, alternating")
-    ap.add_argument("--rounds", type=int, default=3, help="off / on pairs per mode with --mesh-cull")
+    ap.add_argument("--rounds", type=int, default=3, help="off / on pairs per mode with --mesh-cull / --task-cull")
+    ap.add_argument("--task-cull", action="store_true", help="cluster / task modes with the TASK_CULL switch off and on, alternating, then the pass-through kernels on C4")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("raster_modes_bench.py needs a CUDA device")
@@ -176,6 +223,18 @@ def main():
     cache = scene_cache.SceneCache(os.path.join(golden, "kitten.z.cache"))
     if not np.array_equal(cache.section("meshes"), s.meshes):
         sys.exit("kitten.z.cache does not hold the meshes of kitten.nvcg")
+    if args.task_cull:
+        modes = [m for m in args.modes.split(",") if m != "indexed"]  # the draw path has no cluster pass
+        geometry = {"vertices": s.vertices, "indices": cache.section("indices")}
+        for r in range(args.rounds):
+            for mode in modes:
+                for on in ((False, True) if r % 2 == 0 else (True, False)):
+                    print(json.dumps(run_mode(mode, s, geometry, args, task_cull=on)), flush=True)
+        card_info = card()
+        for line in passthrough_c4(args):
+            line.update(card_info)
+            print(json.dumps(line), flush=True)
+        return
     if args.mesh_cull:
         modes = [m for m in args.modes.split(",") if m != "indexed"]  # mesh.vert has no per-triangle stage
         geometry = {"vertices": s.vertices, "indices": cache.section("indices")}
