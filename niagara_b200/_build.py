@@ -41,14 +41,14 @@ def needs_build():
     return any(os.path.exists(d) and os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False, defines=(), out=None):
-    """Compiles every CUDA source for sm_90a into niagara_b200/libniagara_cull.so (or `out`, for tuning variants
-    selected at run time with NVC_LIB_PATH)."""
+def build(force=False, verbose=False, out=None):
+    """Compiles every CUDA source for sm_90a into niagara_b200/libniagara_cull.so (or `out`, e.g. a build of another
+    revision for an A/B, selected at run time with NVC_LIB_PATH)."""
     out = out or LIB_PATH
     if not force and out == LIB_PATH and not needs_build():
         return LIB_PATH
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    cmd = [_nvcc()] + NVCC_FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] + srcs + ["-ldl"]
+    cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out] + srcs + ["-ldl"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + res.stdout + res.stderr)

@@ -57,11 +57,7 @@ __device__ __forceinline__ uint4 ldg_u4(const void* p)
 
 // Read-once streams (meshlet bounds, task commands): read-only path with an L2 evict-first policy, so that the hundreds of MB a pass
 // streams through do not push the depth pyramid / footprint image (read at random, many times) out of L2.
-// NVC_STREAM_HINTS=0 builds plain read-only loads (A/B variant).
-#ifndef NVC_STREAM_HINTS
-#define NVC_STREAM_HINTS 1
-#endif
-#if NVC_STREAM_HINTS && !defined(NVC_EMU)
+#if !defined(NVC_EMU)
 __device__ __forceinline__ uint64_t stream_policy()
 {
 	uint64_t pol;
@@ -86,12 +82,7 @@ __device__ __forceinline__ float4 ldg_stream_f4(const void* p, uint64_t pol)
 	asm("ld.global.nc.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
 	return v;
 }
-__device__ __forceinline__ void prefetch_l2(const void* p)
-{
-	asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-}
 #else
-__device__ __forceinline__ void prefetch_l2(const void*) {}
 __device__ __forceinline__ uint64_t stream_policy() { return 0; }
 __device__ __forceinline__ uint2 ldg_stream_u2(const void* p, uint64_t) { return __ldg(reinterpret_cast<const uint2*>(p)); }
 __device__ __forceinline__ uint32_t ldg_stream_u32(const void* p, uint64_t) { return __ldg(reinterpret_cast<const uint32_t*>(p)); }
@@ -103,37 +94,6 @@ __device__ __forceinline__ float4 ldg_stream_f4(const void* p, uint64_t) { retur
 // not expressible at the PTX level (ptxas sees through register copies), see DESIGN.md "things that did not help".
 typedef NvcCullData ClusterConsts;
 
-// Tuning knobs: software prefetch of the next chunk's loads is not used (its extra registers cost occupancy); registers
-// are capped at 40 so that 6 CTAs (48 warps) are resident per SM.
-#ifndef NVC_ALIVE_FLATTEN
-#define NVC_ALIVE_FLATTEN 1
-#endif
-#ifndef NVC_UNIFORM_FLATTEN
-#define NVC_UNIFORM_FLATTEN 1
-#endif
-// NVC_SMEM_ITEMS=1 (early pass with visibility tracking): instead of re-deriving item -> (command, lane) per chunk with redux / ballot /
-// select_bit64, every command lane scatters its set visibility bits ONCE per batch into a per-warp shared-memory table; chunks then
-// read one 16-bit entry per item.  Validated under the CPU emulation (tests/test_kernels_emulated.py); not timed.
-#ifndef NVC_SMEM_ITEMS
-#define NVC_SMEM_ITEMS 0
-#endif
-// NVC_PDL=1: programmatic dependent launch.  Every frame kernel starts with cudaGridDependencySynchronize() and is launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization, so the CTAs of pass N+1 are scheduled while pass N drains (the five passes of a
-// frame are 5 launches: ramp-up / drain is a measurable share).  Compiles; not timed (build-time variant).
-#ifndef NVC_PDL
-#define NVC_PDL 0
-#endif
-#if NVC_PDL && !defined(NVC_EMU)
-#define NVC_GRID_DEPENDENCY_SYNC() cudaGridDependencySynchronize()
-#else
-#define NVC_GRID_DEPENDENCY_SYNC() ((void)0)
-#endif
-#ifndef NVC_CLUSTER_MIN_BLOCKS
-#define NVC_CLUSTER_MIN_BLOCKS 6
-#endif
-#ifndef NVC_PYRAMID_MIN_BLOCKS
-#define NVC_PYRAMID_MIN_BLOCKS 7
-#endif
 
 struct HiZLoad
 {
@@ -213,18 +173,16 @@ __device__ __forceinline__ void hiz_stage_wait(uint64_t* bar)
 constexpr int kDrawBlock = 256;
 // Draws per thread.  The idea of DPT > 1: all DPT x 3 draw loads are in flight together and the fixed part of a CTA (dependent
 // mesh-head load, the block's atomicAdd round trip, completion ticket, turnover) is paid once per DPT x 256 draws.  The registers
-// and the longer tail of DPT > 1 cost more than the amortisation wins, so the default stays at one draw per thread.
-#ifndef NVC_DRAW_PER_THREAD
-#define NVC_DRAW_PER_THREAD 1
-#endif
-constexpr int kDPT = NVC_DRAW_PER_THREAD;
+// and the longer tail of DPT > 1 cost more than the amortisation wins, so the kernel runs one draw per thread.  Its per-draw
+// state stays in length-kDPT arrays walked by the phase loops: written as scalars, the compiler merges the branches of the
+// mesh-head loads and of the sphere tests, which changes the generated code of every instantiation.
+constexpr int kDPT = 1;
 constexpr uint32_t kDrawQueue = 128; // undecided draws per block that go through the shared queue (more: evaluated in place)
-constexpr uint32_t kDrawStage = 512 * kDPT > 1536 ? 1536 : 512 * kDPT; // commands staged per block before the coalesced write-out (static shared memory <= 48 KB)
+constexpr uint32_t kDrawStage = 512; // commands staged per block before the coalesced write-out (static shared memory <= 48 KB)
 
 template <bool LATE, bool TASK>
 __global__ void __launch_bounds__(kDrawBlock) drawcull_kernel(const DrawCullParams p)
 {
-	NVC_GRID_DEPENDENCY_SYNC(); // nothing of the previous pass (scratch counters, dvb, pyramid) is touched before this point
 	__shared__ uint32_t s_warp_total[kDrawBlock / 32];
 	__shared__ uint32_t s_block_base, s_block_total;
 	__shared__ uint32_t s_is_last;
@@ -809,7 +767,9 @@ __device__ __forceinline__ void update_visibility_bits(uint32_t* mvb, bool activ
 constexpr int kClusterBlock = 256;
 constexpr int kClusterWarps = kClusterBlock / 32;
 constexpr int kStage = 256; // staged cluster indices per warp before one global atomicAdd + coalesced write-out
-constexpr uint32_t kItems = 512; // NVC_SMEM_ITEMS: items of one batch that fit the per-warp table (larger batches take the generic path)
+// Software prefetch of the next chunk's loads is not used (its extra registers cost occupancy); registers are capped at 40
+// so that 6 CTAs (48 warps) are resident per SM.
+constexpr int kClusterMinBlocks = 6;
 
 __device__ __forceinline__ void flush_stage(const ClusterParams& p, uint32_t* stage, uint32_t& nst)
 {
@@ -829,18 +789,55 @@ __device__ __forceinline__ void flush_stage(const ClusterParams& p, uint32_t* st
 	nst = 0;
 }
 
+// clustersubmit.comp.glsl:25-45 as the epilogue of a cluster pass; every thread of the 256-thread block calls it at the end.
+// The CTA that takes the last ticket on cluster_done publishes the cluster count, pads cib with ~0u up to the next multiple
+// of 256 (blockDim == 256 == clustersubmit's local_size_x), and zeroes the pass's scratch counters for the next pass.
+// TASKOUT: the survivors went to the task payloads, so there is no cluster list to publish or pad.
+template <bool TASKOUT>
+__device__ __forceinline__ void clustersubmit_epilogue(const ClusterParams& p, uint32_t& s_is_last)
+{
+	const uint32_t tid = threadIdx.x;
+	__threadfence();
+	__syncthreads();
+	if (tid == 0)
+		s_is_last = atomicAdd(&p.scratch->cluster_done, 1u) == gridDim.x - 1;
+	__syncthreads();
+	if (!s_is_last)
+		return;
+	__threadfence();
+
+	if (!TASKOUT)
+	{
+		const uint32_t clusterCount = *reinterpret_cast<volatile uint32_t*>(&p.scratch->cluster_counter);
+		const uint32_t count = min(clusterCount, p.cluster_limit);
+		if (tid == 0)
+		{
+			p.cluster_count4[0] = clusterCount;
+			p.cluster_count4[1] = NVC_CLUSTER_TILE;
+			p.cluster_count4[2] = min((count + 255) / 256, NVC_MAX_DISPATCH_GROUPS);
+			p.cluster_count4[3] = 256 / NVC_CLUSTER_TILE;
+		}
+		const uint32_t boundary = (count + 255) & ~255u;
+		if (count + tid < boundary)
+			p.cluster_indices[count + tid] = ~0u;
+	}
+	__syncthreads();
+	if (tid == 0)
+	{
+		p.scratch->cluster_counter = 0; // replaces vkCmdFillBuffer(ccb, 0, 4, 0) niagara.cpp:1586
+		p.scratch->cluster_done = 0;
+		p.scratch->cluster_batch = 0;
+	}
+}
+
 template <bool LATE, bool STAGED>
-__global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) clustercull_kernel(const ClusterParams p)
+__global__ void __launch_bounds__(kClusterBlock, kClusterMinBlocks) clustercull_kernel(const ClusterParams p)
 {
 	__shared__ uint32_t s_stage[kClusterWarps][kStage];
-#if NVC_SMEM_ITEMS
-	__shared__ uint16_t s_items[LATE ? 1 : kClusterWarps][LATE ? 1 : kItems];
-#endif
 	__shared__ uint32_t s_is_last;
 	__shared__ __align__(8) uint64_t s_hiz_bar;
 	extern __shared__ __align__(16) float s_hiz[]; // coarse Hi-Z mips (STAGED only)
 
-	NVC_GRID_DEPENDENCY_SYNC();
 	if (STAGED)
 		hiz_stage_begin(p.hiz, s_hiz, &s_hiz_bar); // the copy overlaps the first batch's command / geometry loads
 	bool hiz_ready = !STAGED;
@@ -851,11 +848,6 @@ __global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) cluster
 	const uint32_t lane = tid & 31u, warp = tid >> 5;
 	uint32_t* stage = s_stage[warp];
 	uint32_t nst = 0;
-#if NVC_SMEM_ITEMS
-	uint16_t* const item_table = s_items[LATE ? 0 : warp];
-#else
-	uint16_t* const item_table = nullptr;
-#endif
 
 	// the reference dispatches (X,64,1) groups from dccb+4 (niagara.cpp:1599): commandId < X * 64
 	const uint32_t ncmd = p.command_count4[1] * 64u;
@@ -888,7 +880,7 @@ __global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) cluster
 		// Early pass with visibility tracking: only meshlets whose bit is set can survive (clustercull.comp.glsl:91-92), and
 		// the bits are known up front — so flatten the SET BITS of every command's 64-bit visibility window instead of
 		// all its lanes.  Meshlets that were invisible last frame then cost nothing (no geometry fetch, no arithmetic).
-		const bool alive_flatten = NVC_ALIVE_FLATTEN && !LATE && cd.clusterOcclusionEnabled == 1 && cd.postPass == 0;
+		const bool alive_flatten = !LATE && cd.clusterOcclusionEnabled == 1 && cd.postPass == 0;
 		uint32_t amask_lo = 0, amask_hi = 0;
 		uint32_t eff_count = c_count;
 		if (alive_flatten)
@@ -924,34 +916,14 @@ __global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) cluster
 		// all 32 commands carry the same meshlet count (instanced meshes at one LOD, the synthetic scenes): then
 		// command = item / count, one multiply-high with a per-batch reciprocal (exact: item < 2^11, count <= 64)
 		const uint32_t count0 = __shfl_sync(0xffffffffu, eff_count, 0);
-		const bool uniform = NVC_UNIFORM_FLATTEN && count0 >= 2 && __all_sync(0xffffffffu, eff_count == count0); // (count 1: the reciprocal would not fit)
+		const bool uniform = count0 >= 2 && __all_sync(0xffffffffu, eff_count == count0); // (count 1: the reciprocal would not fit)
 		const uint32_t recip = uniform ? 0xffffffffu / count0 + 1u : 0u; // ceil(2^32 / count0)
-
-		// NVC_SMEM_ITEMS: item table of this batch, entry = (command lane << 6) | meshlet lane, in flattened order
-		const bool use_table = NVC_SMEM_ITEMS && !LATE && alive_flatten && total <= kItems;
-		if (use_table)
-		{
-			uint16_t* tbl = item_table;
-			__syncwarp(); // the previous batch's readers are done
-			uint32_t k = excl;
-			for (uint32_t m = amask_lo; m; m &= m - 1u)
-				tbl[k++] = uint16_t((lane << 6) | uint32_t(__ffs(int(m)) - 1));
-			for (uint32_t m = amask_hi; m; m &= m - 1u)
-				tbl[k++] = uint16_t((lane << 6) | uint32_t(32 + __ffs(int(m)) - 1));
-			__syncwarp();
-		}
 
 		// item -> command mapping of the chunk starting at `base` (executed by all lanes)
 		auto map_chunk = [&](uint32_t base) -> ItemRef {
 			const uint32_t item = base + lane;
 			uint32_t j;
-			uint32_t table_entry = 0;
-			if (use_table)
-			{
-				table_entry = item < total ? uint32_t(item_table[item]) : 0u;
-				j = table_entry >> 6;
-			}
-			else if (uniform)
+			if (uniform)
 				j = __umulhi(item, recip);
 			else if (nz_prefix)
 			{
@@ -979,8 +951,8 @@ __global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) cluster
 			r.active = item < total;
 			r.drawId = __shfl_sync(0xffffffffu, c_draw, j);
 			r.lateVis = __shfl_sync(0xffffffffu, c_late, j);
-			uint32_t mgi = use_table ? (table_entry & 63u) : item - __shfl_sync(0xffffffffu, excl, j); // rank of the item inside its command
-			if (alive_flatten && !use_table)
+			uint32_t mgi = item - __shfl_sync(0xffffffffu, excl, j); // rank of the item inside its command
+			if (alive_flatten)
 			{
 				// the rank-th SET bit of the command's visibility window is the meshlet's lane index
 				const uint32_t mlo = __shfl_sync(0xffffffffu, amask_lo, j), mhi = __shfl_sync(0xffffffffu, amask_hi, j);
@@ -1040,35 +1012,7 @@ __global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) cluster
 	if (!hiz_ready)
 		hiz_stage_wait(&s_hiz_bar); // never leave the CTA while the bulk copy may still be writing its shared memory
 
-	// ---- last-block epilogue: clustersubmit.comp.glsl:25-45 ----
-	__threadfence();
-	__syncthreads();
-	if (tid == 0)
-		s_is_last = atomicAdd(&p.scratch->cluster_done, 1u) == gridDim.x - 1;
-	__syncthreads();
-	if (!s_is_last)
-		return;
-	__threadfence();
-
-	uint32_t clusterCount = *reinterpret_cast<volatile uint32_t*>(&p.scratch->cluster_counter);
-	uint32_t count = min(clusterCount, p.cluster_limit);
-	if (tid == 0)
-	{
-		p.cluster_count4[0] = clusterCount;
-		p.cluster_count4[1] = NVC_CLUSTER_TILE;
-		p.cluster_count4[2] = min((count + 255) / 256, NVC_MAX_DISPATCH_GROUPS);
-		p.cluster_count4[3] = 256 / NVC_CLUSTER_TILE;
-	}
-	uint32_t boundary = (count + 255) & ~255u;
-	if (count + tid < boundary) // blockDim == 256 == the reference's local_size_x
-		p.cluster_indices[count + tid] = ~0u;
-	__syncthreads();
-	if (tid == 0)
-	{
-		p.scratch->cluster_counter = 0; // replaces vkCmdFillBuffer(ccb, 0, 4, 0) niagara.cpp:1586
-		p.scratch->cluster_done = 0;
-		p.scratch->cluster_batch = 0;
-	}
+	clustersubmit_epilogue<false>(p, s_is_last);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1086,30 +1030,16 @@ __global__ void __launch_bounds__(kClusterBlock, NVC_CLUSTER_MIN_BLOCKS) cluster
 //     meshlet_compute on full warps, 32 at a time — so the result is bit-identical to the exact kernel's.
 // ------------------------------------------------------------------------------------------------------
 
-#ifndef NVC_FILTER_MIN_BLOCKS
-#define NVC_FILTER_MIN_BLOCKS 4
-#endif
-// resident CTAs per SM of the EARLY filtered kernel (no occlusion stage: fewer live registers; its shared-memory block is sized below)
-#ifndef NVC_FILTER_MIN_BLOCKS_EARLY
-#define NVC_FILTER_MIN_BLOCKS_EARLY 4
-#endif
-#ifndef NVC_FILTER_ITEMS
-#define NVC_FILTER_ITEMS 896
-#endif
-#ifndef NVC_FILTER_PIPELINE
-#define NVC_FILTER_PIPELINE 2
-#endif
-// NVC_FILTER_BATCH_PREFETCH=1: batch tickets are taken one batch ahead, and the next batch's task commands (then its draws) are
-// pulled into L2 while the current batch is evaluated, so the command -> draw -> record chain of the next batch starts from L2.
-#ifndef NVC_FILTER_BATCH_PREFETCH
-#define NVC_FILTER_BATCH_PREFETCH 0
-#endif
+// resident CTAs per SM of the late and of the EARLY filtered kernel (no occlusion stage: fewer live registers; its shared-memory
+// block is sized below)
+constexpr int kFilterMinBlocks = 4;
+constexpr int kFilterMinBlocksEarly = 4;
 constexpr int kFFlush = 128;           // cluster indices written out per flush: ONE atomicAdd + four coalesced 128-byte stores per warp
 constexpr int kFStage = kFFlush + 32;  // staged cluster indices per warp (a chunk appends <= 32 before the next flush)
 constexpr int kFQueue = 64;            // undecided items per warp (drained 32 at a time)
 // early pass: (command lane, meshlet lane) of every flattened item of one (sub-)batch; batches with more set bits are
 // processed as four sub-batches of 8 commands (<= 512 items)
-constexpr uint32_t kFItems = NVC_FILTER_ITEMS;
+constexpr uint32_t kFItems = 896;
 static_assert(kFItems >= 8u * 64u, "a sub-batch of 8 commands (<= 64 meshlets each) must fit the item table");
 
 // One block of shared memory per warp: every field sits at a compile-time offset from the warp's base address.
@@ -1131,12 +1061,11 @@ static_assert(sizeof(FilterWarpShared<false>) * (256 / 32) + 16 <= 48 * 1024, "s
 // BF: clusterBackfaceEnabled as a compile-time fact (0 / 1; -1 = read at run time).  With it the cone arithmetic is
 // scheduled between the Hi-Z load and its use instead of behind a branch.
 template <bool LATE, bool FP, bool TRACK, bool TASKOUT, int BF>
-__global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : NVC_FILTER_MIN_BLOCKS_EARLY) clustercull_filter_kernel(const ClusterParams p)
+__global__ void __launch_bounds__(kClusterBlock, LATE ? kFilterMinBlocks : kFilterMinBlocksEarly) clustercull_filter_kernel(const ClusterParams p)
 {
 	__shared__ FilterWarpShared<LATE> sh_all[kClusterWarps];
 	__shared__ uint32_t s_is_last;
 
-	NVC_GRID_DEPENDENCY_SYNC();
 	const NvcCullData& cd = p.cull;
 	const ClusterConsts& cc = cd;
 	const FilterConsts& fc = p.filter;
@@ -1244,35 +1173,14 @@ __global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : 
 		__syncwarp();
 	};
 
-#if NVC_FILTER_BATCH_PREFETCH
-	uint32_t batch = 0, batch_next = 0;
-	if (lane == 0)
-	{
-		batch = atomicAdd(&p.scratch->cluster_batch, 1u);
-		batch_next = atomicAdd(&p.scratch->cluster_batch, 1u);
-	}
-	batch = __shfl_sync(0xffffffffu, batch, 0);
-	batch_next = __shfl_sync(0xffffffffu, batch_next, 0);
-#endif
 	for (;;)
 	{
-#if NVC_FILTER_BATCH_PREFETCH
-		if (batch >= nbatch)
-			break;
-		uint32_t ticket = 0;
-		if (lane == 0)
-			ticket = atomicAdd(&p.scratch->cluster_batch, 1u); // consumed at the end of this batch
-		const uint32_t cid_next = batch_next * 32u + lane;
-		if (batch_next < nbatch && cid_next < ncmd)
-			prefetch_l2(p.task_commands + cid_next);
-#else
 		uint32_t batch = 0;
 		if (lane == 0)
 			batch = atomicAdd(&p.scratch->cluster_batch, 1u);
 		batch = __shfl_sync(0xffffffffu, batch, 0);
 		if (batch >= nbatch)
 			break;
-#endif
 
 		// ---- per command: load, visibility window, transform record ----
 		const uint32_t cid = batch * 32u + lane;
@@ -1341,8 +1249,8 @@ __global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : 
 				recip = uniform ? 0xffffffffu / count0 + 1u : 0u;
 			}
 
-			// item -> (j, mgi) and the meshlet's loads for the chunk starting at `b`.  Software pipeline (NVC_FILTER_PIPELINE):
-			// the loads of chunk k+1 are issued before chunk k is evaluated, so their DRAM latency overlaps its arithmetic.
+			// item -> (j, mgi) and the meshlet's loads for the chunk starting at `b`.  Software pipeline: the loads of chunks k+1
+			// and k+2 are issued before chunk k is evaluated, so their DRAM latency overlaps its arithmetic.
 			// Carried state: one packed word (j | mgi << 8 | old visibility bit << 30 | active << 31) + the 12 loaded bytes.
 			auto fetch = [&](uint32_t b, uint32_t& jm, uint2& b0, uint32_t& b1) {
 				const uint32_t item = b + lane;
@@ -1396,44 +1304,24 @@ __global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : 
 					load_meshlet_cull<true>(p, ids.x + mgi, spol, b0, b1);
 			};
 
-			// NVC_FILTER_PIPELINE = prefetch distance in chunks (0: none).  Distance 2 keeps two chunks (2 x 384 bytes per warp from
-			// the meshlet cull view, 2 x 768 from the 24-byte records) in
-			// flight: with one, a chunk's arithmetic (~0.6 us at 8 warps per scheduler) is shorter than the DRAM latency under load
+			// Prefetch distance 2 chunks: two chunks (2 x 384 bytes per warp from the meshlet cull view, 2 x 768 from the 24-byte
+			// records) in flight.  With one, a chunk's arithmetic (~0.6 us at 8 warps per scheduler) is shorter than the DRAM
+			// latency under load; with none, the whole latency is exposed.  n_*: chunk k+1, m_*: chunk k+2.
 			uint32_t n_jm = 0, n_b1 = 0, m_jm = 0, m_b1 = 0;
 			uint2 n_b0 = make_uint2(0u, 0u), m_b0 = make_uint2(0u, 0u);
-#if NVC_FILTER_PIPELINE >= 1
 			if (run_total)
 				fetch(0u, n_jm, n_b0, n_b1);
-#endif
-#if NVC_FILTER_PIPELINE >= 2
 			if (run_total > 32u)
 				fetch(32u, m_jm, m_b0, m_b1);
-#endif
 			for (uint32_t base = 0; base < run_total; base += 32)
 			{
-#if NVC_FILTER_PIPELINE >= 2
 				const uint32_t jm = n_jm, b1 = n_b1;
 				const uint2 b0 = n_b0;
 				n_jm = m_jm, n_b0 = m_b0, n_b1 = m_b1;
 				if (base + 64u < run_total)
 					fetch(base + 64u, m_jm, m_b0, m_b1);
-#elif NVC_FILTER_PIPELINE == 1
-				const uint32_t jm = n_jm, b1 = n_b1;
-				const uint2 b0 = n_b0;
-				if (base + 32u < run_total)
-					fetch(base + 32u, n_jm, n_b0, n_b1);
-#else
-				fetch(base, n_jm, n_b0, n_b1);
-				const uint32_t jm = n_jm, b1 = n_b1;
-				const uint2 b0 = n_b0;
-				(void)m_jm, (void)m_b1, (void)m_b0;
-#endif
 				const bool active = (jm >> 31) != 0u;
 				const uint32_t j = jm & 31u;
-#if NVC_FILTER_BATCH_PREFETCH
-				if (base == 96u && batch_next < nbatch && cid_next < ncmd) // the commands have reached L2 by now: pull the draws
-					prefetch_l2(p.draws + __ldg(&p.task_commands[cid_next].drawId));
-#endif
 
 				// ---- the command's record, the meshlet's visibility bit ----
 				const CmdRecord& rec = recs[j];
@@ -1503,10 +1391,6 @@ __global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : 
 			__syncwarp(); // records visible to the whole warp
 			run(std::false_type(), total, excl, incl);
 		}
-#if NVC_FILTER_BATCH_PREFETCH
-		batch = batch_next;
-		batch_next = __shfl_sync(0xffffffffu, ticket, 0);
-#endif
 	}
 	while (nq)
 		drain(min(nq, 32u));
@@ -1519,38 +1403,7 @@ __global__ void __launch_bounds__(kClusterBlock, LATE ? NVC_FILTER_MIN_BLOCKS : 
 			atomicAdd(&p.scratch->filter_undecided, (unsigned long long)stat_undecided);
 	}
 
-	// ---- last-block epilogue: clustersubmit.comp.glsl:25-45 ----
-	__threadfence();
-	__syncthreads();
-	if (tid == 0)
-		s_is_last = atomicAdd(&p.scratch->cluster_done, 1u) == gridDim.x - 1;
-	__syncthreads();
-	if (!s_is_last)
-		return;
-	__threadfence();
-
-	if (!TASKOUT)
-	{
-		uint32_t clusterCount = *reinterpret_cast<volatile uint32_t*>(&p.scratch->cluster_counter);
-		uint32_t count = min(clusterCount, p.cluster_limit);
-		if (tid == 0)
-		{
-			p.cluster_count4[0] = clusterCount;
-			p.cluster_count4[1] = NVC_CLUSTER_TILE;
-			p.cluster_count4[2] = min((count + 255) / 256, NVC_MAX_DISPATCH_GROUPS);
-			p.cluster_count4[3] = 256 / NVC_CLUSTER_TILE;
-		}
-		uint32_t boundary = (count + 255) & ~255u;
-		if (count + tid < boundary)
-			p.cluster_indices[count + tid] = ~0u;
-	}
-	__syncthreads();
-	if (tid == 0)
-	{
-		p.scratch->cluster_counter = 0;
-		p.scratch->cluster_done = 0;
-		p.scratch->cluster_batch = 0;
-	}
+	clustersubmit_epilogue<TASKOUT>(p, s_is_last);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1673,35 +1526,7 @@ __global__ void __launch_bounds__(kPassBlock) clustercull_passthrough_kernel(con
 		__syncthreads(); // s_count / s_offset / s_warp_total are reused by the next tile
 	}
 
-	// ---- last-block epilogue: clustersubmit.comp.glsl:25-45 (as in clustercull_kernel) ----
-	__threadfence();
-	__syncthreads();
-	if (tid == 0)
-		s_is_last = atomicAdd(&p.scratch->cluster_done, 1u) == gridDim.x - 1;
-	__syncthreads();
-	if (!s_is_last)
-		return;
-	__threadfence();
-
-	const uint32_t clusterCount = *reinterpret_cast<volatile uint32_t*>(&p.scratch->cluster_counter);
-	const uint32_t count = min(clusterCount, p.cluster_limit);
-	if (tid == 0)
-	{
-		p.cluster_count4[0] = clusterCount;
-		p.cluster_count4[1] = NVC_CLUSTER_TILE;
-		p.cluster_count4[2] = min((count + 255) / 256, NVC_MAX_DISPATCH_GROUPS);
-		p.cluster_count4[3] = 256 / NVC_CLUSTER_TILE;
-	}
-	const uint32_t boundary = (count + 255) & ~255u;
-	if (count + tid < boundary) // blockDim == 256 == clustersubmit's local_size_x
-		p.cluster_indices[count + tid] = ~0u;
-	__syncthreads();
-	if (tid == 0)
-	{
-		p.scratch->cluster_counter = 0;
-		p.scratch->cluster_done = 0;
-		p.scratch->cluster_batch = 0;
-	}
+	clustersubmit_epilogue<false>(p, s_is_last);
 }
 
 // meshlet.task.glsl:144-148: for every command c < command_count4[1] * 64, all 64 lanes write payload.clusterIndices[lane] =
@@ -1760,15 +1585,16 @@ __device__ __forceinline__ float reduce2x2(const float* src, uint32_t sw, uint32
 	return fminf(fminf(src[y0 * spitch + x0], src[y0 * spitch + x1]), fminf(src[y1 * spitch + x0], src[y1 * spitch + x1]));
 }
 
-template <bool EXACT>
 // 7 resident CTAs per SM = 1036 slots: the 1024 tiles of a 2048^2 pyramid (4096^2 depth target) run as ONE wave
-__global__ void __launch_bounds__(kPyrBlock, NVC_PYRAMID_MIN_BLOCKS) pyramid_kernel(const PyramidParams p)
+constexpr int kPyrMinBlocks = 7;
+
+template <bool EXACT>
+__global__ void __launch_bounds__(kPyrBlock, kPyrMinBlocks) pyramid_kernel(const PyramidParams p)
 {
 	__shared__ float s_a[kPyrTile * kPyrTile];             // level 0 tile, later levels 2, 4, 6
 	__shared__ float s_b[(kPyrTile / 2) * (kPyrTile / 2)]; // levels 1, 3, 5
 	__shared__ uint32_t s_is_last;
 
-	NVC_GRID_DEPENDENCY_SYNC();
 	const HiZDesc& hz = p.hiz;
 	const uint32_t tid = threadIdx.x;
 	const uint32_t tile_x = blockIdx.x * kPyrTile, tile_y = blockIdx.y * kPyrTile;
@@ -2600,24 +2426,6 @@ cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uin
 	return cudaGetLastError();
 }
 
-#if NVC_PDL && !defined(NVC_EMU)
-template <typename P, typename... Extra>
-static cudaError_t launch_pdl(void (*kernel)(P, Extra...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, const P& p, Extra... extra)
-{
-	cudaLaunchConfig_t cfg = {};
-	cfg.gridDim = grid;
-	cfg.blockDim = block;
-	cfg.dynamicSmemBytes = smem;
-	cfg.stream = stream;
-	cudaLaunchAttribute attr[1];
-	attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-	attr[0].val.programmaticStreamSerializationAllowed = 1;
-	cfg.attrs = attr;
-	cfg.numAttrs = 1;
-	return cudaLaunchKernelEx(&cfg, kernel, p, extra...);
-}
-#endif
-
 // ------------------------------------------------------------------------------------------------------
 // footprint image: F_l(i, j) = min over the clamped 2 x 2 footprint (i, i+1) x (j, j+1) of mip l, i in [-1, w-1]
 // (see HiZDesc).  With it a sampler access whose four texels all count (fract != 0 on both axes — the only case the
@@ -2641,7 +2449,6 @@ __host__ __device__ __forceinline__ uint32_t footprint_row_groups(uint32_t h)
 // loads per row.  Both were instruction bound.)
 __global__ void __launch_bounds__(256) footprint_kernel(const HiZDesc hz, float* __restrict__ fp, uint32_t total)
 {
-	NVC_GRID_DEPENDENCY_SYNC();
 	(void)total;
 	// block -> (level, row group): uniform walk over <= 16 levels
 	uint32_t l = hz.fp_first, rg = blockIdx.x;
@@ -2714,12 +2521,8 @@ cudaError_t launch_footprint(const HiZDesc& hiz, float* fp, uint32_t total, cuda
 	uint32_t blocks = 0;
 	for (uint32_t l = hiz.fp_first; l < hiz.levels; ++l)
 		blocks += footprint_row_groups(hiz.height >> l ? hiz.height >> l : 1u);
-#if NVC_PDL && !defined(NVC_EMU)
-	return launch_pdl(footprint_kernel, dim3(blocks), dim3(256), 0, stream, hiz, fp, total);
-#else
 	footprint_kernel<<<blocks, 256, 0, stream>>>(hiz, fp, total);
 	return cudaGetLastError();
-#endif
 }
 
 cudaError_t launch_drawcull(const DrawCullParams& p, bool late, bool task, cudaStream_t stream)
@@ -2727,24 +2530,8 @@ cudaError_t launch_drawcull(const DrawCullParams& p, bool late, bool task, cudaS
 	uint32_t blocks = (p.cull.drawCount + kDrawBlock * kDPT - 1) / (kDrawBlock * kDPT);
 	if (blocks == 0)
 		blocks = 1;
-#if NVC_PDL && !defined(NVC_EMU)
 	void (*kernel)(DrawCullParams) = late ? (task ? drawcull_kernel<true, true> : drawcull_kernel<true, false>) : (task ? drawcull_kernel<false, true> : drawcull_kernel<false, false>);
-	return launch_pdl(kernel, dim3(blocks), dim3(kDrawBlock), 0, stream, p);
-#endif
-	if (late)
-	{
-		if (task)
-			drawcull_kernel<true, true><<<blocks, kDrawBlock, 0, stream>>>(p);
-		else
-			drawcull_kernel<true, false><<<blocks, kDrawBlock, 0, stream>>>(p);
-	}
-	else
-	{
-		if (task)
-			drawcull_kernel<false, true><<<blocks, kDrawBlock, 0, stream>>>(p);
-		else
-			drawcull_kernel<false, false><<<blocks, kDrawBlock, 0, stream>>>(p);
-	}
+	kernel<<<blocks, kDrawBlock, 0, stream>>>(p);
 	return cudaGetLastError();
 }
 
@@ -2774,24 +2561,12 @@ cudaError_t launch_clustercull(const ClusterParams& p, bool late, uint32_t block
 			kernel = late ? (p.hiz.fp ? pick_filter_kernel<true, true, true>(track, bf) : pick_filter_kernel<true, false, true>(track, bf)) : pick_filter_kernel<false, false, true>(track, bf);
 		else
 			kernel = late ? (p.hiz.fp ? pick_filter_kernel<true, true, false>(track, bf) : pick_filter_kernel<true, false, false>(track, bf)) : pick_filter_kernel<false, false, false>(track, bf);
-#if NVC_PDL && !defined(NVC_EMU)
-		return launch_pdl(kernel, dim3(blocks), dim3(kClusterBlock), 0, stream, p);
-#else
 		kernel<<<blocks, kClusterBlock, 0, stream>>>(p);
 		return cudaGetLastError();
-#endif
 	}
 	const uint32_t stage_bytes = late ? hiz_stage_bytes(p.hiz) : 0u;
-#if NVC_PDL && !defined(NVC_EMU)
 	void (*kernel)(ClusterParams) = late ? (stage_bytes ? clustercull_kernel<true, true> : clustercull_kernel<true, false>) : clustercull_kernel<false, false>;
-	return launch_pdl(kernel, dim3(blocks), dim3(kClusterBlock), stage_bytes, stream, p);
-#endif
-	if (late && stage_bytes)
-		clustercull_kernel<true, true><<<blocks, kClusterBlock, stage_bytes, stream>>>(p);
-	else if (late)
-		clustercull_kernel<true, false><<<blocks, kClusterBlock, 0, stream>>>(p);
-	else
-		clustercull_kernel<false, false><<<blocks, kClusterBlock, 0, stream>>>(p);
+	kernel<<<blocks, kClusterBlock, stage_bytes, stream>>>(p);
 	return cudaGetLastError();
 }
 
@@ -2804,10 +2579,8 @@ cudaError_t launch_taskcull(const ClusterParams& p, bool late, NvcMeshTaskPayloa
 		q.emit_counts = emit_counts;
 		return launch_clustercull(q, late, blocks, stream);
 	}
-	if (late)
-		taskcull_kernel<true><<<blocks, kClusterBlock, 0, stream>>>(p, payloads, emit_counts);
-	else
-		taskcull_kernel<false><<<blocks, kClusterBlock, 0, stream>>>(p, payloads, emit_counts);
+	void (*kernel)(ClusterParams, NvcMeshTaskPayload*, uint32_t*) = late ? taskcull_kernel<true> : taskcull_kernel<false>;
+	kernel<<<blocks, kClusterBlock, 0, stream>>>(p, payloads, emit_counts);
 	return cudaGetLastError();
 }
 
@@ -2832,13 +2605,8 @@ cudaError_t launch_pyramid(const PyramidParams& p, cudaStream_t stream)
 	// 16-byte loads of the depth rows / 8-byte stores of mip 0 need aligned bases (row pitches are multiples of 4 / 2
 	// texels whenever a full 64-texel tile exists)
 	q.vector_ok = (reinterpret_cast<uintptr_t>(p.depth) & 15u) == 0 && (reinterpret_cast<uintptr_t>(p.hiz.texels) & 7u) == 0 && (p.depth_width & 3u) == 0;
-#if NVC_PDL && !defined(NVC_EMU)
-	return launch_pdl(exact ? pyramid_kernel<true> : pyramid_kernel<false>, grid, dim3(kPyrBlock), 0, stream, q);
-#endif
-	if (exact)
-		pyramid_kernel<true><<<grid, kPyrBlock, 0, stream>>>(q);
-	else
-		pyramid_kernel<false><<<grid, kPyrBlock, 0, stream>>>(q);
+	void (*kernel)(PyramidParams) = exact ? pyramid_kernel<true> : pyramid_kernel<false>;
+	kernel<<<grid, kPyrBlock, 0, stream>>>(q);
 	return cudaGetLastError();
 }
 

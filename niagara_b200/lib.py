@@ -102,7 +102,8 @@ SIGNATURES = [
 
 
 def library_path():
-    # NVC_LIB_PATH selects a tuning variant built with _build.build(defines=..., out=...); default = the product build
+    # NVC_LIB_PATH selects another build of the library (e.g. one of another revision, made with _build.build(out=...), for an
+    # A/B); default = the product build
     return os.environ.get("NVC_LIB_PATH") or _build.LIB_PATH
 
 

@@ -21,19 +21,18 @@ OUT = os.path.join(HERE, "_build", "emu")
 _LIB = None
 
 
-def load(defines=()):
-    """Builds (when stale) and loads the emulated library.  `defines`: extra -D macros (kernel variants)."""
+def load():
+    """Builds (when stale) and loads the emulated library."""
     global _LIB
-    key = "_".join(defines).replace("=", "")
-    so = os.path.join(OUT, "libniagara_cull_emu%s.so" % (("_" + key) if key else ""))
-    if not defines and _LIB is not None:
+    so = os.path.join(OUT, "libniagara_cull_emu.so")
+    if _LIB is not None:
         return _LIB
     os.makedirs(OUT, exist_ok=True)
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(EMU, f) for f in ("gen_emu.py", "emu.cpp", "emu_stubs.cpp")] + [os.path.join(EMU, "include", f) for f in os.listdir(os.path.join(EMU, "include"))] + [os.path.join(ROOT, "include", "niagara_cull.h")]
     if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         for name in ("nvc_kernels", "nvc_api"):
             subprocess.run(["python3", os.path.join(EMU, "gen_emu.py"), os.path.join(CSRC, name + ".cu"), os.path.join(OUT, name + ".cpp")], check=True)
-        cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I", os.path.join(EMU, "include"), "-I", CSRC] + ["-D" + d for d in defines]
+        cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I", os.path.join(EMU, "include"), "-I", CSRC]
         cmd += ["-o", so, os.path.join(OUT, "nvc_kernels.cpp"), os.path.join(OUT, "nvc_api.cpp"), os.path.join(EMU, "emu.cpp"), os.path.join(EMU, "emu_stubs.cpp"), os.path.join(CSRC, "nvc_host.cpp")]
         subprocess.run(cmd, check=True)
     lib = ctypes.CDLL(so)
@@ -41,8 +40,7 @@ def load(defines=()):
         if hasattr(lib, name):
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = restype, argtypes
-    if not defines:
-        _LIB = lib
+    _LIB = lib
     return lib
 
 
@@ -53,9 +51,9 @@ def _p(a):
 class EmuPath(oracle_lib.OraclePath):
     """OraclePath's buffers, every pass executed by the product's kernels under the SIMT emulation."""
 
-    def __init__(self, *args, defines=(), prepare_meshes=True, prepare_hiz=True, **kwargs):
+    def __init__(self, *args, prepare_meshes=True, prepare_hiz=True, **kwargs):
         super().__init__(*args, **kwargs)
-        self.emu = load(defines)
+        self.emu = load()
         self.ctx = ctypes.c_void_p()
         limits = layout.Limits(self.limits.task_wglimit, self.limits.cluster_limit)
         assert self.emu.nvc_create(0, ctypes.byref(limits), ctypes.byref(self.ctx)) == 0

@@ -1,7 +1,7 @@
 """CPU-only: the PRODUCT's CUDA kernels executed under the SIMT emulation of tests/cuda_emu (nvc_kernels.cu + nvc_api.cu compiled
 by g++, same C ABI, host pointers) against the oracle — the -m gpu parity suite in miniature for a machine without a GPU.  It checks
 kernel logic (indexing, block / warp scans, flattening, compaction, staging, epilogues, arithmetic order); what only hardware can
-show (memory model, timing) stays with the GPU tests.  Build-time variants of the cluster kernels are covered too."""
+show (memory model, timing) stays with the GPU tests."""
 import ctypes
 import os
 
@@ -13,9 +13,9 @@ import oracle_lib
 from niagara_b200 import host, layout, scenes
 
 
-def _pair(s, defines=(), threads=4, **kw):
+def _pair(s, threads=4, **kw):
     o = oracle_lib.OraclePath(s.meshes, s.meshlets, s.draws, *s.screen, threads=threads, **kw)
-    e = emu_lib.EmuPath(s.meshes, s.meshlets, s.draws, *s.screen, defines=defines, **kw)
+    e = emu_lib.EmuPath(s.meshes, s.meshlets, s.draws, *s.screen, **kw)
     o.set_visibility_bits(s.visibility_bits)
     e.set_visibility_bits(s.visibility_bits)
     return o, e
@@ -42,8 +42,8 @@ def _compare_clusters(o, e, what):
     assert np.array_equal(o.mvb, e.mvb), what
 
 
-def _frames(s, frames=2, toggles=None, cluster_backface=True, cameras=None, post_passes=False, defines=(), **kw):
-    o, e = _pair(s, defines=defines, **kw)
+def _frames(s, frames=2, toggles=None, cluster_backface=True, cameras=None, post_passes=False, **kw):
+    o, e = _pair(s, **kw)
     emitted = 0
     for f in range(frames):
         if cameras:
@@ -233,18 +233,28 @@ def test_hostile_inputs(golden_dir):
         _frames(s, frames=2, toggles=dict(culling=False))
 
 
-@pytest.mark.parametrize(
-    "defines",
-    [("NVC_ALIVE_FLATTEN=0",), ("NVC_UNIFORM_FLATTEN=0",), ("NVC_ALIVE_FLATTEN=0", "NVC_UNIFORM_FLATTEN=0"), ("NVC_SMEM_ITEMS=1",), ("NVC_FILTER_ITEMS=512",), ("NVC_FILTER_PIPELINE=1",), ("NVC_FILTER_PIPELINE=0",)],
-)
-def test_build_time_variants(golden_dir, defines):
-    """the compile-time variants of the cluster kernels (the flatten strategies; filtered kernel: the smallest
-    item table (512 entries), so that the dense batches of the kitten scenes take the 8-command sub-batch path, and the meshlet prefetch distances 1 and 0)"""
-    assert _frames(_kp(golden_dir, 3000), defines=defines) > 300
-    assert _frames(scenes.config4_scene(draw_count=6000, screen=(512, 512)), defines=defines, cmd_capacity=12000) > 3000
-    # several frames with a moving camera: the early pass sees sparse, changing visibility masks
+def test_kitten_config4_and_moving_camera_frames(golden_dir):
+    """the cluster kernels' item -> command mappings on the kitten / pirate and C4 scenes and on frames with a moving camera,
+    where the early pass sees sparse, changing visibility masks"""
+    assert _frames(_kp(golden_dir, 3000)) > 300
+    assert _frames(scenes.config4_scene(draw_count=6000, screen=(512, 512)), cmd_capacity=12000) > 3000
     cams = [host.make_camera((0, 0, 0)), host.make_camera((12, -4, 9), host.quat_from_axis_angle((0, 1, 0), 0.35)), host.make_camera((25, 3, -14), host.quat_from_axis_angle((0.1, 1, 0), 0.9))]
-    assert _frames(_kp(golden_dir, 2500, screen=(800, 600)), frames=4, cameras=cams, defines=defines) > 300
+    assert _frames(_kp(golden_dir, 2500, screen=(800, 600)), frames=4, cameras=cams) > 300
+    # task commands with taskCount 0 between non-empty ones (drawcull never writes them): without visibility tracking the
+    # filtered kernel then maps items to commands by the scan search
+    s = _kp(golden_dir, 2500)
+    cd = s.cull_data(cluster_occlusion=False)
+    o, e = _pair(s)
+    for p in (o, e):
+        p.pyramid(s.depth)
+        p.cull(cd, True)
+    _compare_draw(o, e, True, "empty commands")
+    for p in (o, e):
+        p.dcb.view(np.uint32)[2 : 5 * int(p.dccb[0]) : 15] = 0  # taskCount of every third command
+    o.render_clusters(cd, True, cluster_backface=True)
+    e.render_clusters(cd, True, cluster_backface=True)
+    _compare_clusters(o, e, "empty commands")
+    assert 0 < int(e.ccb[0]) < int(np.minimum(e.dcb.view(np.uint32)[2 : 5 * int(e.dccb[0]) : 5], 64).sum())
 
 
 def test_tma_staged_hiz(golden_dir):
@@ -323,14 +333,13 @@ def _guarded(arr):
 _guarded.keep = []
 
 
-@pytest.mark.parametrize("defines", [(), ("NVC_SMEM_ITEMS=1",)])
-def test_no_access_past_buffer_ends(golden_dir, defines):
+def test_no_access_past_buffer_ends(golden_dir):
     """Every device buffer of the passes (draws, meshes, meshlets, dvb, dcb, dccb, cib, ccb, mvb, depth, pyramid) ends at a
     PROT_NONE page while the emulated kernels run two frames + the small kernels: an overrun would be a SIGSEGV."""
     s = _kp(golden_dir, 2047, screen=(333, 217))  # odd sizes: ragged last blocks / tiles
     o = oracle_lib.OraclePath(s.meshes, s.meshlets, s.draws, *s.screen, threads=4)
     o.set_visibility_bits(s.visibility_bits)
-    e = emu_lib.EmuPath(s.meshes, s.meshlets, s.draws, *s.screen, defines=defines, prepare_meshes=False)
+    e = emu_lib.EmuPath(s.meshes, s.meshlets, s.draws, *s.screen, prepare_meshes=False)
     e.set_visibility_bits(s.visibility_bits)
     for name in ("meshes", "meshlets", "draws", "dvb", "dcb", "dccb", "cib", "ccb", "mvb", "pyramid_texels"):
         setattr(e, name, _guarded(getattr(e, name)))

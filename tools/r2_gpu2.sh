@@ -13,7 +13,6 @@ q > $O/bench_default.json; summ default < $O/bench_default.json
 NVC_PREPARE_HIZ=0 q > $O/bench_nofp.json; summ nofp < $O/bench_nofp.json
 NVC_DRAW_FILTER=1 q > $O/bench_drawfilter.json; summ drawfilter < $O/bench_drawfilter.json
 NVC_CLUSTER_FILTER=0 q > $O/bench_exact.json; summ exact < $O/bench_exact.json
-for v in nopipe nohints bpf bpf_fb3 fb3 fb5 pdl; do NVC_LIB_PATH=$PWD/niagara_b200/variant_$v.so q > $O/bench_$v.json; summ $v < $O/bench_$v.json; done
 python bench.py --workload C2 --steps 30 --warmup 3 --no-e2e --no-cpu-baseline --no-extras 2>>$O/err.log | tail -1 > $O/bench_c2.json; summ C2 < $O/bench_c2.json
 echo "== ncu full: every kernel of one frame"
 timeout 900 ncu --set full --clock-control none --import-source on -s 30 -c 6 -f -o $O/prof_frame python bench.py --steps 2 --warmup 3 --no-e2e --no-cpu-baseline --no-extras > $O/ncu_full.log 2>&1; tail -2 $O/ncu_full.log | cut -c1-200

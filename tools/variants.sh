@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B of tuning variants built with _build.build(defines=..., out=niagara_b200/variant_<name>.so)
+# A/B of libraries built with _build.build(out=niagara_b200/variant_<name>.so), e.g. from other revisions
 for v in "$@"; do
   echo "== variant $v"
   NVC_LIB_PATH=$PWD/niagara_b200/variant_$v.so python bench.py --steps 20 --warmup 3 --no-e2e --no-cpu-baseline 2>&1 | python -c "
