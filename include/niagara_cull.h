@@ -618,6 +618,31 @@ NVC_API int nvc_set_task_cull(NvcContext* ctx, int enabled);
 NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count,
     const uint32_t* meshletdata, uint32_t meshletdata_words, NvcMeshlet* meshlets, uint32_t meshlet_count, uint32_t* rejected);
 
+/* Builds and packs the meshlets of every LOD of a whole Mesh[] on the device, bit-identical to what the reference's cooker
+ * stores (scene.cpp:270-276 appendMesh -> appendMeshlets with clrt off: meshopt_buildMeshlets(64 vertices, 96 triangles, cone
+ * weight 0.25), meshopt_optimizeMeshletLevel(level 1) per meshlet, then appendMeshlet's packing and bounds):
+ *   vertices / vertex_count   device: the scene's Vertex[] (vb); positions are the fp16 vx, vy, vz
+ *   indices / index_count     device: the mesh-local indices of every LOD (ib)
+ *   host_meshes / mesh_count  host: vertexOffset, vertexCount, lodCount and lods[].indexOffset / indexCount are read
+ *   meshes                    device out: host_meshes with lods[l].meshletOffset / meshletCount set for l < lodCount
+ *   meshlets, meshletdata     device out: Meshlet[] and meshletdata, meshlets of mesh 0 LOD 0 first; may be NULL with capacity 0
+ *   totals4                   device out: meshlets needed, words needed (saturated at 2^32 - 1), LODs rejected, overflow flag
+ * The bytes of a meshlet's last triangle word past triangleCount * 3 are 0 (the reference leaves whatever its scratch buffer
+ * held there; nothing reads them).  A LOD with an index >= its mesh's vertexCount is rejected: it gets meshletCount 0, is
+ * counted in totals4[2], and none of its vertices is read.  When the meshlets or words needed exceed meshlet_capacity or
+ * meshletdata_capacity, totals4[3] is 1 and neither array is written (meshes is); nvc_cook_meshlets_capacity gives sizes
+ * that always suffice.  NVC_ERROR_INVALID_ARGUMENT: lodCount > 8, an indexCount not a multiple of 3, or a LOD index range or
+ * mesh vertex range outside indices / vertices.  Scratch is context-owned and grows as needed, and the call synchronises the
+ * device before it enqueues its kernels on `stream`: call it at load time, outside stream capture.  Not covered: the
+ * cooker's ray-tracing LOD of clrt builds (meshopt_buildMeshletsSpatial and meshletvtx0), the LOD chain itself
+ * (meshopt_simplifyWithAttributes: the index ranges are inputs), and appending to existing Meshlet[] / meshletdata. */
+NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices,
+    uint32_t index_count, const NvcMesh* host_meshes, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity,
+    uint32_t* meshletdata, uint32_t meshletdata_capacity, uint32_t* totals4);
+/* Host: capacities nvc_cook_meshlets never exceeds for these meshes: per LOD meshopt_buildMeshletsBound(indexCount, 64, 96)
+ * meshlets and indexCount + ceil(indexCount / 4) + that bound words.  NVC_ERROR_INVALID_ARGUMENT when a lodCount > 8. */
+NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out);
+
 #ifdef __cplusplus
 } /* extern "C" */
 

@@ -1,6 +1,10 @@
 // nvc_api.cu — the C ABI declared in include/niagara_cull.h (context, argument validation, launches).
 #include "nvc_internal.h"
 #include "nvc_filter.cuh"
+#include "nvc_meshlets.cuh"
+
+#include <algorithm>
+#include <vector>
 
 #include <stdio.h>
 #include <stdlib.h>
@@ -244,6 +248,8 @@ NVC_API void nvc_destroy(NvcContext* ctx)
 		cudaFree(ctx->meshlet_cone);
 	if (ctx->hiz_fp)
 		cudaFree(ctx->hiz_fp);
+	if (ctx->cook_scratch)
+		cudaFree(ctx->cook_scratch);
 	delete ctx;
 }
 
@@ -743,6 +749,142 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
 		return NVC_ERROR_INVALID_ARGUMENT;
 	cudaError_t e = nvc::launch_cook_meshlet_bounds(vertices, vertex_count, meshletdata, meshletdata_words, meshlets, meshlet_count, rejected, static_cast<cudaStream_t>(stream));
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_meshlet_bounds");
+}
+
+NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out)
+{
+	if ((mesh_count && !host_meshes) || !meshlets_out || !words_out)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	uint64_t meshlets = 0, words = 0;
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		if (host_meshes[i].lodCount > NVC_MAX_LODS)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		for (uint32_t l = 0; l < host_meshes[i].lodCount; ++l)
+		{
+			meshlets += nvc::cook::meshlets_bound(host_meshes[i].lods[l].indexCount);
+			words += nvc::cook::words_bound(host_meshes[i].lods[l].indexCount);
+		}
+	}
+	*meshlets_out = meshlets > 0xffffffffull ? 0xffffffffu : uint32_t(meshlets);
+	*words_out = words;
+	return NVC_OK;
+}
+
+NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices, uint32_t index_count,
+    const NvcMesh* host_meshes, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity, uint32_t* meshletdata,
+    uint32_t meshletdata_capacity, uint32_t* totals4)
+{
+	if (!ctx || !totals4 || (mesh_count && (!host_meshes || !meshes)) || (meshlet_capacity && !meshlets) || (meshletdata_capacity && !meshletdata))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+
+	// plan: one job per LOD in mesh then LOD order, each with its own scratch ranges
+	std::vector<nvc::cook::CookJob> jobs;
+	uint64_t tri = 0, vtx = 0, idx = 0, slot = 0;
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		const NvcMesh& mesh = host_meshes[i];
+		if (mesh.lodCount > NVC_MAX_LODS || uint64_t(mesh.vertexOffset) + mesh.vertexCount > vertex_count)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		for (uint32_t l = 0; l < mesh.lodCount; ++l)
+		{
+			const NvcMeshLod& lod = mesh.lods[l];
+			if (lod.indexCount % 3 != 0 || uint64_t(lod.indexOffset) + lod.indexCount > index_count)
+				return NVC_ERROR_INVALID_ARGUMENT;
+			if (lod.indexCount && !indices)
+				return NVC_ERROR_INVALID_ARGUMENT;
+			nvc::cook::CookJob job = { i, l, lod.indexOffset, lod.indexCount, mesh.vertexOffset, mesh.vertexCount, tri, vtx, idx, slot };
+			jobs.push_back(job);
+			tri += lod.indexCount / 3;
+			vtx += mesh.vertexCount;
+			idx += lod.indexCount;
+			slot += nvc::cook::meshlets_bound(lod.indexCount);
+		}
+	}
+	if (jobs.size() && !vertices)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (slot > 0xffffffffull)
+		return NVC_ERROR_INVALID_ARGUMENT; // meshlet slots are counted in 32 bits
+	const uint32_t job_count = uint32_t(jobs.size());
+	// the longest jobs start first; outputs are placed by job index, so the order does not change them
+	std::vector<uint32_t> order(job_count);
+	for (uint32_t j = 0; j < job_count; ++j)
+		order[j] = j;
+	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+
+	// scratch layout, 256-byte aligned sub-allocations
+	size_t bytes = 0;
+	auto take = [&](size_t n) {
+		size_t at = bytes;
+		bytes += (n + 255) & ~size_t(255);
+		return at;
+	};
+	size_t o_jobs = take(job_count * sizeof(nvc::cook::CookJob)), o_order = take(job_count * 4ull);
+	size_t o_cones = take(tri * 24u), o_counts = take(vtx * 4u), o_offsets = take(vtx * 4u), o_used = take(vtx * 2u);
+	size_t o_data = take(idx * 4u), o_mlv = take(idx * 4u), o_mlt = take(idx), o_emitted = take(tri);
+	size_t o_nodes = take(tri * 24u), o_kdi = take(tri * 4u), o_records = take(slot * 16u);
+	size_t o_words = take(slot * 4u), o_min = take(slot * 4u), o_sdata = take(slot * 4u);
+	size_t o_jm = take(job_count * 4ull), o_jf = take(job_count * 4ull);
+
+	DeviceGuard guard(ctx->device);
+	// the previous call may still use the scratch, and the copies below are not ordered with `stream`
+	cudaError_t e = cudaDeviceSynchronize();
+	if (e == cudaSuccess && bytes > ctx->cook_scratch_bytes)
+	{
+		cudaFree(ctx->cook_scratch);
+		ctx->cook_scratch = nullptr;
+		ctx->cook_scratch_bytes = 0;
+		e = cudaMalloc(&ctx->cook_scratch, bytes);
+		if (e == cudaErrorMemoryAllocation)
+			return NVC_ERROR_OUT_OF_MEMORY;
+		if (e == cudaSuccess)
+			ctx->cook_scratch_bytes = bytes;
+	}
+	char* base = static_cast<char*>(ctx->cook_scratch);
+	if (e == cudaSuccess && job_count)
+		e = cudaMemcpy(base + o_jobs, jobs.data(), job_count * sizeof(nvc::cook::CookJob), cudaMemcpyHostToDevice);
+	if (e == cudaSuccess && job_count)
+		e = cudaMemcpy(base + o_order, order.data(), job_count * 4ull, cudaMemcpyHostToDevice);
+	if (e == cudaSuccess && mesh_count)
+		e = cudaMemcpy(meshes, host_meshes, size_t(mesh_count) * sizeof(NvcMesh), cudaMemcpyHostToDevice);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, "nvc_cook_meshlets");
+
+	nvc::CookArgs a;
+	a.vertices = vertices;
+	a.indices = indices;
+	a.jobs = reinterpret_cast<const nvc::cook::CookJob*>(base + o_jobs);
+	a.order = reinterpret_cast<const uint32_t*>(base + o_order);
+	a.job_count = job_count;
+	a.slot_count = uint32_t(slot);
+	a.cones = reinterpret_cast<float*>(base + o_cones);
+	a.adj_counts = reinterpret_cast<uint32_t*>(base + o_counts);
+	a.adj_offsets = reinterpret_cast<uint32_t*>(base + o_offsets);
+	a.adj_data = reinterpret_cast<uint32_t*>(base + o_data);
+	a.used = reinterpret_cast<int16_t*>(base + o_used);
+	a.emitted = reinterpret_cast<uint8_t*>(base + o_emitted);
+	a.kd_nodes = reinterpret_cast<uint32_t*>(base + o_nodes);
+	a.kd_index = reinterpret_cast<uint32_t*>(base + o_kdi);
+	a.ml_vertices = reinterpret_cast<uint32_t*>(base + o_mlv);
+	a.ml_triangles = reinterpret_cast<uint8_t*>(base + o_mlt);
+	a.ml_records = reinterpret_cast<uint4*>(base + o_records);
+	a.job_meshlets = reinterpret_cast<uint32_t*>(base + o_jm);
+	a.job_first = reinterpret_cast<uint32_t*>(base + o_jf);
+	a.slot_words = reinterpret_cast<uint32_t*>(base + o_words);
+	a.slot_min = reinterpret_cast<uint32_t*>(base + o_min);
+	a.slot_data = reinterpret_cast<uint32_t*>(base + o_sdata);
+	a.meshes = meshes;
+	a.meshlets = meshlets;
+	a.meshlet_capacity = meshlet_capacity;
+	a.meshletdata = meshletdata;
+	a.meshletdata_capacity = meshletdata_capacity;
+	a.totals4 = totals4;
+	e = nvc::launch_cook_meshlets(a, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_meshlets");
 }
 
 } // extern "C"

@@ -46,6 +46,9 @@ struct NvcContext
 	uint32_t hiz_fp_first = 0; // first mip with a footprint image (env NVC_FP_FIRST_LEVEL)
 	uint32_t hiz_fp_offset[NVC_MAX_HIZ_LEVELS] = {};
 	bool hiz_fp_valid = false; // set by nvc_depth_pyramid, cleared by nvc_prepare_hiz
+	// nvc_cook_meshlets: job table and per-job scratch, grown as needed
+	void* cook_scratch = nullptr;
+	size_t cook_scratch_bytes = 0;
 };
 
 namespace nvc
@@ -217,6 +220,45 @@ cudaError_t launch_raster_depth_indexed(const float* projection16, const NvcCull
     const NvcMeshDraw* draws, const uint32_t* indices, uint32_t index_count, const NvcVertex* vertices, uint32_t vertex_count, float* depth, uint32_t width, uint32_t height, uint32_t* stats4,
     uint32_t blocks, cudaStream_t stream);
 cudaError_t launch_cook_meshlet_bounds(const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* meshletdata, uint32_t meshletdata_words, NvcMeshlet* meshlets, uint32_t meshlet_count, uint32_t* rejected, cudaStream_t stream);
+namespace cook
+{
+struct CookJob;
+}
+
+// nvc_cook_meshlets: the jobs (one per mesh LOD, in mesh then LOD order), the order the build kernel takes them in, and the
+// scratch the host planned for them (nvc_meshlets.cuh).  Every pointer is device memory.
+struct CookArgs
+{
+	const NvcVertex* vertices;
+	const uint32_t* indices;
+	const cook::CookJob* jobs;
+	const uint32_t* order; // job indices, largest first
+	uint32_t job_count;
+	uint32_t slot_count; // meshlet slots of all jobs (sum of their bounds)
+	float* cones;        // 6 per triangle
+	uint32_t* adj_counts; // per vertex: live triangles
+	uint32_t* adj_offsets;
+	uint32_t* adj_data;   // per index
+	int16_t* used;        // per vertex
+	uint8_t* emitted;     // per triangle
+	uint32_t* kd_nodes;   // 2 nodes of 3 words per triangle
+	uint32_t* kd_index;   // per triangle
+	uint32_t* ml_vertices; // per index; also the triangle areas before the greedy loop
+	uint8_t* ml_triangles; // per index
+	uint4* ml_records;     // per slot: vertex offset, triangle offset, vertex count, triangle count
+	uint32_t* job_meshlets; // per job: meshlets built
+	uint32_t* job_first;    // per job: first output meshlet
+	uint32_t* slot_words;   // per slot: meshletdata words (0 for an unused slot)
+	uint32_t* slot_min;     // per slot: minVertex
+	uint32_t* slot_data;    // per slot: dataOffset
+	NvcMesh* meshes;
+	NvcMeshlet* meshlets;
+	uint32_t meshlet_capacity;
+	uint32_t* meshletdata;
+	uint32_t meshletdata_capacity;
+	uint32_t* totals4;
+};
+cudaError_t launch_cook_meshlets(const CookArgs& a, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);
 cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream);

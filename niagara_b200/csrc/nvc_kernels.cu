@@ -10,6 +10,7 @@
 #include "nvc_internal.h"
 #include "nvc_math.cuh"
 #include "nvc_cook.cuh"
+#include "nvc_meshlets.cuh"
 #include "nvc_tma.cuh"
 #include "nvc_filter.cuh"
 
@@ -2355,6 +2356,581 @@ cudaError_t launch_cook_meshlet_bounds(const NvcVertex* vertices, uint32_t verte
 	if (meshlet_count == 0)
 		return cudaSuccess;
 	cook_meshlet_bounds_kernel<<<(meshlet_count + 127u) / 128u, 128, 0, stream>>>(vertices, vertex_count, meshletdata, meshletdata_words, meshlets, meshlet_count, rejected);
+	return cudaGetLastError();
+}
+
+// N4: meshlet building and packing (csrc/nvc_meshlets.cuh)
+namespace
+{
+
+constexpr uint32_t kCookWarps = 4;        // jobs per block of the build kernel
+constexpr uint32_t kCookScanThreads = 256; // the one block of the scan kernel
+
+__device__ __forceinline__ uint32_t cook_warp_inclusive(uint32_t v, uint32_t lane)
+{
+	for (uint32_t d = 1; d < 32; d <<= 1)
+	{
+		uint32_t o = __shfl_up_sync(0xffffffffu, v, d);
+		v += lane >= d ? o : 0u;
+	}
+	return v;
+}
+
+// Orders scores as floats do, with -0 == +0 and NaN above everything
+__device__ __forceinline__ uint32_t cook_score_key(float s)
+{
+	if (s != s)
+		return 0xffffffffu;
+	uint32_t u = cook::float_bits(s == 0.0f ? 0.0f : s);
+	return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// getNeighborTriangle (clusterizer.cpp:302-362) for the whole warp.  Candidate k is the k-th (meshlet vertex, live
+// neighbour) pair in the reference's loop order; lanes take k = lane, lane + 32, ...  The reference keeps the best
+// (priority, score) on a strict '<', i.e. among the lowest priority the first candidate of the least score -- unless the
+// first candidate of that priority scores NaN, which no later candidate then replaces.  So two minima are reduced:
+// (priority, k) and (priority, score, k).
+__device__ uint32_t cook_neighbor(uint32_t lane, const cook::Building& m, const cook::Cone& mc, const uint32_t* mlv, const uint32_t* indices, const uint32_t* counts,
+    const uint32_t* offsets, const uint32_t* data, const float* cones, const int16_t* used, float expected_radius, uint32_t* s_prefix, uint32_t* s_mv)
+{
+	const uint32_t full = 0xffffffffu;
+	uint32_t v0 = 0, v1 = 0, c0 = 0, c1 = 0;
+	if (lane < m.vertex_count)
+	{
+		v0 = mlv[m.vertex_offset + lane];
+		c0 = counts[v0];
+	}
+	if (lane + 32 < m.vertex_count)
+	{
+		v1 = mlv[m.vertex_offset + lane + 32];
+		c1 = counts[v1];
+	}
+	uint32_t p0 = cook_warp_inclusive(c0, lane);
+	uint32_t p1 = cook_warp_inclusive(c1, lane) + __shfl_sync(full, p0, 31);
+	if (lane == 0)
+		s_prefix[0] = 0;
+	s_prefix[lane + 1] = p0;
+	s_prefix[lane + 33] = p1;
+	s_mv[lane] = v0;
+	s_mv[lane + 32] = v1;
+	__syncwarp();
+	const uint32_t total = s_prefix[m.vertex_count];
+
+	uint32_t fp = 5, fk = 0, fs = 0, ft = cook::kNone; // first candidate of the least priority, its score bits
+	uint32_t bp = 5, bs = 0, bk = 0, bt = cook::kNone; // least (priority, score, k)
+	for (uint32_t k = lane; k < total; k += 32)
+	{
+		uint32_t lo = 0, hi = m.vertex_count;
+		while (hi - lo > 1)
+		{
+			uint32_t mid = (lo + hi) >> 1;
+			if (s_prefix[mid] <= k)
+				lo = mid;
+			else
+				hi = mid;
+		}
+		uint32_t tri = data[offsets[s_mv[lo]] + (k - s_prefix[lo])];
+		uint32_t a = indices[tri * 3 + 0], b = indices[tri * 3 + 1], c = indices[tri * 3 + 2];
+		uint32_t extra = (used[a] < 0) + (used[b] < 0) + (used[c] < 0);
+		uint32_t priority;
+		if (extra == 0)
+			priority = 0;
+		else if (counts[a] == 1 || counts[b] == 1 || counts[c] == 1)
+			priority = 1;
+		else if ((counts[a] == 2) + (counts[b] == 2) + (counts[c] == 2) >= 2)
+			priority = 1 + extra;
+		else
+			priority = 2 + extra;
+		if (priority > bp)
+			continue;
+		const float* tc = cones + size_t(tri) * 6u;
+		float distance = cook::point_distance(tc, mc.px, mc.py, mc.pz);
+		float spread = cook::add(cook::add(cook::mul(tc[3], mc.nx), cook::mul(tc[4], mc.ny)), cook::mul(tc[5], mc.nz));
+		float score = cook::meshlet_score(distance, spread, expected_radius);
+		uint32_t key = cook_score_key(score);
+		if (priority < fp) // k increases within a lane: the first of a priority is the first seen
+		{
+			fp = priority;
+			fk = k;
+			fs = cook::float_bits(score);
+			ft = tri;
+		}
+		if (priority < bp || (priority == bp && key < bs))
+		{
+			bp = priority;
+			bs = key;
+			bk = k;
+			bt = tri;
+		}
+	}
+	for (int d = 16; d > 0; d >>= 1)
+	{
+		uint32_t op = __shfl_xor_sync(full, fp, d), ok = __shfl_xor_sync(full, fk, d), os = __shfl_xor_sync(full, fs, d), ot = __shfl_xor_sync(full, ft, d);
+		if (op < fp || (op == fp && ok < fk))
+			fp = op, fk = ok, fs = os, ft = ot;
+		uint32_t bp2 = __shfl_xor_sync(full, bp, d), bs2 = __shfl_xor_sync(full, bs, d), bk2 = __shfl_xor_sync(full, bk, d), bt2 = __shfl_xor_sync(full, bt, d);
+		if (bp2 < bp || (bp2 == bp && (bs2 < bs || (bs2 == bs && bk2 < bk))))
+			bp = bp2, bs = bs2, bk = bk2, bt = bt2;
+	}
+	__syncwarp(); // s_prefix / s_mv are rewritten by the next call
+	if (fp == 5)
+		return cook::kNone;
+	float first = cook::bits_float(fs);
+	return first != first ? ft : bt;
+}
+
+// One warp per (mesh, LOD) job: meshopt_buildMeshletsFlex (clusterizer.cpp:1035-1224) with the parameters of
+// meshopt_buildMeshlets(64, 96, 0.25).  Jobs are taken in a.order (largest first); results are placed by job index.
+__global__ void __launch_bounds__(kCookWarps * 32) cook_build_kernel(const CookArgs a)
+{
+	__shared__ uint32_t s_seeds[kCookWarps][cook::kMaxSeeds];
+	__shared__ uint32_t s_prefix[kCookWarps][2 * 32 + 1];
+	__shared__ uint32_t s_mv[kCookWarps][cook::kMaxVertices];
+	__shared__ uint32_t s_bn[kCookWarps][cook::kMaxVertices];
+	__shared__ uint32_t s_bl[kCookWarps][cook::kMaxVertices];
+	__shared__ float s_bs[kCookWarps][cook::kMaxVertices];
+	const uint32_t full = 0xffffffffu;
+	const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+	const uint32_t w = blockIdx.x * kCookWarps + warp;
+	if (w >= a.job_count)
+		return;
+	const uint32_t j = a.order[w];
+	const cook::CookJob job = a.jobs[j];
+	const uint32_t* indices = a.indices + job.index_offset;
+	const uint32_t index_count = job.index_count, faces = index_count / 3, vertex_count = job.vertex_count;
+
+	// an index outside the mesh: the LOD gets no meshlets (the reference asserts)
+	bool bad = false;
+	for (uint32_t i = lane; i < index_count; i += 32)
+		bad = bad || indices[i] >= vertex_count;
+	if (__any_sync(full, bad) || faces == 0)
+	{
+		if (lane == 0)
+		{
+			a.job_meshlets[j] = 0;
+			if (faces != 0)
+				atomicAdd(a.totals4 + 2, 1u);
+		}
+		return;
+	}
+
+	float* cones = a.cones + job.tri * 6u;
+	uint32_t* counts = a.adj_counts + job.vtx;
+	uint32_t* offsets = a.adj_offsets + job.vtx;
+	uint32_t* data = a.adj_data + job.idx;
+	int16_t* used = a.used + job.vtx;
+	uint8_t* emitted = a.emitted + job.tri;
+	uint32_t* nodes = a.kd_nodes + job.tri * 6u;
+	uint32_t* kdi = a.kd_index + job.tri;
+	uint32_t* mlv = a.ml_vertices + job.idx;
+	uint8_t* mlt = a.ml_triangles + job.idx;
+	uint4* records = a.ml_records + job.slot;
+	float* areas = reinterpret_cast<float*>(mlv); // free until the greedy loop
+	const NvcVertex* verts = a.vertices + job.vertex_offset;
+
+	// computeTriangleCones (clusterizer.cpp:201-241), areas summed below in triangle order
+	for (uint32_t t = lane; t < faces; t += 32)
+	{
+		cook::V3 p[3];
+		for (int k = 0; k < 3; ++k)
+		{
+			const NvcVertex& v = verts[indices[t * 3 + k]];
+			p[k] = cook::V3{ cook::dequantize_half(v.vx), cook::dequantize_half(v.vy), cook::dequantize_half(v.vz) };
+		}
+		cook::Cone c;
+		areas[t] = cook::triangle_cone(p[0], p[1], p[2], c);
+		float* dst = cones + size_t(t) * 6u;
+		dst[0] = c.px, dst[1] = c.py, dst[2] = c.pz, dst[3] = c.nx, dst[4] = c.ny, dst[5] = c.nz;
+		emitted[t] = 0;
+		kdi[t] = t;
+	}
+	for (uint32_t v = lane; v < vertex_count; v += 32)
+	{
+		counts[v] = 0;
+		used[v] = -1;
+	}
+	__syncwarp();
+	// buildTriangleAdjacency (clusterizer.cpp:40-86): counts, offsets, then a sequential (stable) fill
+	for (uint32_t i = lane; i < index_count; i += 32)
+		atomicAdd(counts + indices[i], 1u);
+	__syncwarp();
+	uint32_t carry = 0;
+	for (uint32_t base = 0; base < vertex_count; base += 32)
+	{
+		uint32_t v = base + lane;
+		uint32_t c = v < vertex_count ? counts[v] : 0u;
+		uint32_t incl = cook_warp_inclusive(c, lane);
+		if (v < vertex_count)
+			offsets[v] = carry + incl - c;
+		carry += __shfl_sync(full, incl, 31);
+	}
+	__syncwarp();
+
+	float expected_radius = 0.0f, corner[3] = { FLT_MAX, FLT_MAX, FLT_MAX };
+	uint32_t initial_seed = cook::kNone;
+	if (lane == 0)
+	{
+		for (uint32_t t = 0; t < faces; ++t)
+		{
+			data[offsets[indices[t * 3 + 0]]++] = t;
+			data[offsets[indices[t * 3 + 1]]++] = t;
+			data[offsets[indices[t * 3 + 2]]++] = t;
+		}
+		float mesh_area = 0.0f;
+		for (uint32_t t = 0; t < faces; ++t)
+			mesh_area = cook::add(mesh_area, areas[t]);
+		float triangle_area_avg = cook::mul(cook::div(mesh_area, float(faces)), 0.5f);
+		expected_radius = cook::mul(cook::root(cook::mul(triangle_area_avg, float(cook::kMaxTriangles))), 0.5f);
+		cook::kd_build(nodes, cones, kdi, faces);
+		for (uint32_t t = 0; t < faces; ++t)
+		{
+			const float* c = cones + size_t(t) * 6u;
+			corner[0] = corner[0] > c[0] ? c[0] : corner[0];
+			corner[1] = corner[1] > c[1] ? c[1] : corner[1];
+			corner[2] = corner[2] > c[2] ? c[2] : corner[2];
+		}
+		float initial_score = FLT_MAX;
+		for (uint32_t t = 0; t < faces; ++t)
+		{
+			float score = cook::point_distance(cones + size_t(t) * 6u, corner[0], corner[1], corner[2]);
+			if (initial_seed == cook::kNone || score < initial_score)
+			{
+				initial_seed = t;
+				initial_score = score;
+			}
+		}
+	}
+	__syncwarp();
+	for (uint32_t v = lane; v < vertex_count; v += 32)
+		offsets[v] -= counts[v];
+	expected_radius = __shfl_sync(full, expected_radius, 0);
+	corner[0] = __shfl_sync(full, corner[0], 0);
+	corner[1] = __shfl_sync(full, corner[1], 0);
+	corner[2] = __shfl_sync(full, corner[2], 0);
+	initial_seed = __shfl_sync(full, initial_seed, 0);
+	__syncwarp();
+
+	uint32_t* seeds = s_seeds[warp];
+	uint32_t seed_count = 0, meshlet_offset = 0;
+	cook::Building m = { 0, 0, 0, 0 };
+	cook::Cone acc = { 0, 0, 0, 0, 0, 0 };
+	for (;;)
+	{
+		cook::Cone mc = cook::meshlet_cone(acc, m.triangle_count);
+		uint32_t best = cook::kNone;
+		if (meshlet_offset == 0 && m.triangle_count == 0)
+			best = initial_seed;
+		else
+			best = cook_neighbor(lane, m, mc, mlv, indices, counts, offsets, data, cones, used, expected_radius, s_prefix[warp], s_mv[warp]);
+		if (best == cook::kNone)
+		{
+			if (lane == 0)
+			{
+				float position[3] = { mc.px, mc.py, mc.pz };
+				float distance = FLT_MAX;
+				cook::kd_nearest(nodes, cones, emitted, position, best, distance);
+			}
+			best = __shfl_sync(full, best, 0);
+		}
+		if (best == cook::kNone)
+			break;
+
+		int best_extra = (used[indices[best * 3 + 0]] < 0) + (used[indices[best * 3 + 1]] < 0) + (used[indices[best * 3 + 2]] < 0);
+		if (m.vertex_count + best_extra > cook::kMaxVertices || m.triangle_count >= cook::kMaxTriangles)
+		{
+			// appendSeedTriangles (clusterizer.cpp:364-430): each meshlet vertex's least-live neighbour, by lanes
+			for (uint32_t i = lane; i < m.vertex_count; i += 32)
+			{
+				uint32_t v = mlv[m.vertex_offset + i];
+				const uint32_t* nb = data + offsets[v];
+				uint32_t n = counts[v], bn = cook::kNone, bl = cook::kNone;
+				for (uint32_t q = 0; q < n; ++q)
+				{
+					uint32_t tri = nb[q];
+					uint32_t live = counts[indices[tri * 3 + 0]] + counts[indices[tri * 3 + 1]] + counts[indices[tri * 3 + 2]];
+					if (live < bl)
+					{
+						bn = tri;
+						bl = live;
+					}
+				}
+				s_bn[warp][i] = bn;
+				s_bl[warp][i] = bl;
+				s_bs[warp][i] = bn == cook::kNone ? 0.0f : cook::point_distance(cones + size_t(bn) * 6u, corner[0], corner[1], corner[2]);
+			}
+			__syncwarp();
+			if (lane == 0)
+			{
+				// pruneSeedTriangles (:432-445) and the cap of :1164
+				uint32_t kept = 0;
+				for (uint32_t i = 0; i < seed_count; ++i)
+				{
+					uint32_t index = seeds[i];
+					seeds[kept] = index;
+					kept += emitted[index] == 0;
+				}
+				seed_count = kept + cook::kAddSeeds <= cook::kMaxSeeds ? kept : cook::kMaxSeeds - cook::kAddSeeds;
+				uint32_t best_seeds[cook::kAddSeeds], best_live[cook::kAddSeeds];
+				float best_score[cook::kAddSeeds];
+				for (uint32_t i = 0; i < cook::kAddSeeds; ++i)
+				{
+					best_seeds[i] = cook::kNone;
+					best_live[i] = cook::kNone;
+					best_score[i] = FLT_MAX;
+				}
+				for (uint32_t i = 0; i < m.vertex_count; ++i)
+				{
+					uint32_t bn = s_bn[warp][i], bl = s_bl[warp][i];
+					float bs = s_bs[warp][i];
+					if (bn == cook::kNone)
+						continue;
+					for (uint32_t q = 0; q < cook::kAddSeeds; ++q)
+						if (bl < best_live[q] || (bl == best_live[q] && bs <= best_score[q]))
+						{
+							best_seeds[q] = bn;
+							best_live[q] = bl;
+							best_score[q] = bs;
+							break;
+						}
+				}
+				for (uint32_t i = 0; i < cook::kAddSeeds; ++i)
+					if (best_seeds[i] != cook::kNone)
+						seeds[seed_count++] = best_seeds[i];
+				uint32_t best_seed = cook::select_seed(seeds, seed_count, indices, cones, counts, corner);
+				best = best_seed != cook::kNone ? best_seed : best;
+			}
+			best = __shfl_sync(full, best, 0);
+			seed_count = __shfl_sync(full, seed_count, 0);
+		}
+
+		uint32_t flushed = 0;
+		if (lane == 0)
+			flushed = cook::append_triangle(m, indices[best * 3 + 0], indices[best * 3 + 1], indices[best * 3 + 2], used, records, meshlet_offset, mlv, mlt) ? 1u : 0u;
+		flushed = __shfl_sync(full, flushed, 0);
+		m.vertex_offset = __shfl_sync(full, m.vertex_offset, 0);
+		m.triangle_offset = __shfl_sync(full, m.triangle_offset, 0);
+		m.vertex_count = __shfl_sync(full, m.vertex_count, 0);
+		m.triangle_count = __shfl_sync(full, m.triangle_count, 0);
+		if (flushed)
+		{
+			meshlet_offset++;
+			acc = cook::Cone{ 0, 0, 0, 0, 0, 0 };
+		}
+		__syncwarp();
+
+		// swap-with-last removal of `best` from its vertices' lists (:1186-1204), one vertex after the other
+		for (int k = 0; k < 3; ++k)
+		{
+			uint32_t v = indices[best * 3 + k];
+			uint32_t* nb = data + offsets[v];
+			uint32_t n = counts[v];
+			for (uint32_t base = 0; base < n; base += 32)
+			{
+				uint32_t i = base + lane;
+				uint32_t hit = __ballot_sync(full, i < n && nb[i] == best);
+				if (hit)
+				{
+					if (lane == uint32_t(__ffs(int(hit)) - 1))
+					{
+						nb[i] = nb[n - 1];
+						counts[v] = n - 1;
+					}
+					break;
+				}
+			}
+			__syncwarp();
+		}
+
+		const float* bc = cones + size_t(best) * 6u;
+		acc.px = cook::add(acc.px, bc[0]);
+		acc.py = cook::add(acc.py, bc[1]);
+		acc.pz = cook::add(acc.pz, bc[2]);
+		acc.nx = cook::add(acc.nx, bc[3]);
+		acc.ny = cook::add(acc.ny, bc[4]);
+		acc.nz = cook::add(acc.nz, bc[5]);
+		if (lane == 0)
+			emitted[best] = 1;
+		__syncwarp();
+	}
+	if (lane == 0)
+	{
+		if (m.triangle_count)
+			records[meshlet_offset++] = make_uint4(m.vertex_offset, m.triangle_offset, m.vertex_count, m.triangle_count);
+		a.job_meshlets[j] = meshlet_offset;
+	}
+}
+
+// the job whose slots hold slot s: the last job starting at or before it
+__device__ __forceinline__ uint32_t cook_job_of_slot(const CookArgs& a, uint32_t s)
+{
+	uint32_t lo = 0, hi = a.job_count;
+	while (hi - lo > 1)
+	{
+		uint32_t mid = (lo + hi) >> 1;
+		if (a.jobs[mid].slot <= s)
+			lo = mid;
+		else
+			hi = mid;
+	}
+	return lo;
+}
+
+// One thread per meshlet: meshopt_optimizeMeshletLevel(level 1), then what appendMeshlet (scene.cpp:26-47) derives from
+// the meshlet's vertices: minVertex, shortRefs and the words it takes.
+__global__ void __launch_bounds__(128) cook_optimize_kernel(const CookArgs a)
+{
+	uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+	if (s >= a.slot_count)
+		return;
+	uint32_t j = cook_job_of_slot(a, s);
+	const cook::CookJob& job = a.jobs[j];
+	if (s - job.slot >= a.job_meshlets[j])
+	{
+		a.slot_words[s] = 0;
+		return;
+	}
+	uint4 r = a.ml_records[s];
+	uint32_t* mv = a.ml_vertices + job.idx + r.x;
+	cook::optimize_meshlet(mv, r.z, a.ml_triangles + job.idx + r.y, r.w);
+	uint32_t lo = ~0u, hi = 0;
+	for (uint32_t i = 0; i < r.z; ++i)
+	{
+		lo = mv[i] < lo ? mv[i] : lo;
+		hi = mv[i] > hi ? mv[i] : hi;
+	}
+	bool short_refs = hi - lo < (1u << 16);
+	a.slot_min[s] = lo;
+	a.slot_words[s] = (short_refs ? (r.z + 1u) / 2u : r.z) + (r.w * 3u + 3u) / 4u;
+}
+
+// exclusive scan of v over the block, returns the block total; s_warp holds 32 words
+__device__ __forceinline__ uint32_t cook_block_exclusive(uint32_t v, uint32_t& total, uint32_t* s_warp)
+{
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	uint32_t incl = cook_warp_inclusive(v, lane);
+	if (lane == 31)
+		s_warp[warp] = incl;
+	__syncthreads();
+	uint32_t before = 0;
+	total = 0;
+	for (uint32_t w = 0; w < kCookScanThreads / 32; ++w)
+	{
+		before += w < warp ? s_warp[w] : 0u;
+		total += s_warp[w];
+	}
+	__syncthreads();
+	return before + incl - v;
+}
+
+// One block: LOD meshlet offsets (scene.cpp:274-275) and meshlet data offsets, both in job order; the totals and the
+// overflow flag.
+__global__ void __launch_bounds__(kCookScanThreads) cook_scan_kernel(const CookArgs a)
+{
+	__shared__ uint32_t s_warp[32];
+	uint64_t carry = 0;
+	for (uint32_t base = 0; base < a.job_count; base += kCookScanThreads)
+	{
+		uint32_t j = base + threadIdx.x;
+		uint32_t n = j < a.job_count ? a.job_meshlets[j] : 0u, total;
+		uint32_t before = cook_block_exclusive(n, total, s_warp);
+		if (j < a.job_count)
+		{
+			uint32_t first = uint32_t(carry + before);
+			a.job_first[j] = first;
+			NvcMeshLod& lod = a.meshes[a.jobs[j].mesh].lods[a.jobs[j].lod];
+			lod.meshletOffset = first;
+			lod.meshletCount = n;
+		}
+		carry += total;
+	}
+	uint64_t meshlets = carry;
+	carry = 0;
+	for (uint32_t base = 0; base < a.slot_count; base += kCookScanThreads)
+	{
+		uint32_t s = base + threadIdx.x;
+		uint32_t n = s < a.slot_count ? a.slot_words[s] : 0u, total;
+		uint32_t before = cook_block_exclusive(n, total, s_warp);
+		if (s < a.slot_count)
+			a.slot_data[s] = uint32_t(carry + before);
+		carry += total;
+	}
+	if (threadIdx.x == 0)
+	{
+		a.totals4[0] = meshlets > 0xffffffffull ? 0xffffffffu : uint32_t(meshlets);
+		a.totals4[1] = carry > 0xffffffffull ? 0xffffffffu : uint32_t(carry);
+		a.totals4[3] = (meshlets > a.meshlet_capacity || carry > a.meshletdata_capacity) ? 1u : 0u;
+	}
+}
+
+// One thread per meshlet: the Meshlet record and its meshletdata words (scene.cpp:26-80), then the bounds of
+// meshopt_computeMeshletBounds from the words just written (cook::meshlet_bounds).  Nothing is written on overflow.
+__global__ void __launch_bounds__(128) cook_pack_kernel(const CookArgs a)
+{
+	uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+	if (s >= a.slot_count || a.totals4[3])
+		return;
+	uint32_t j = cook_job_of_slot(a, s);
+	const cook::CookJob& job = a.jobs[j];
+	uint32_t local = s - uint32_t(job.slot);
+	if (local >= a.job_meshlets[j])
+		return;
+	uint4 r = a.ml_records[s];
+	const uint32_t* mv = a.ml_vertices + job.idx + r.x;
+	const uint8_t* mt = a.ml_triangles + job.idx + r.y;
+	uint32_t lo = a.slot_min[s];
+	uint32_t hi = 0;
+	for (uint32_t i = 0; i < r.z; ++i)
+		hi = mv[i] > hi ? mv[i] : hi;
+	bool short_refs = hi - lo < (1u << 16);
+	uint32_t* dst = a.meshletdata + a.slot_data[s];
+	uint32_t ref_words = short_refs ? (r.z + 1u) / 2u : r.z;
+	for (uint32_t k = 0; k < ref_words; ++k)
+	{
+		if (short_refs)
+			dst[k] = (mv[2 * k] - lo) | (2 * k + 1 < r.z ? (mv[2 * k + 1] - lo) << 16 : 0u);
+		else
+			dst[k] = mv[k] - lo;
+	}
+	uint32_t tri_bytes = r.w * 3u;
+	for (uint32_t wi = 0; wi < (tri_bytes + 3u) / 4u; ++wi)
+	{
+		uint32_t word = 0;
+		for (uint32_t q = 0; q < 4; ++q)
+			word |= (4 * wi + q < tri_bytes ? uint32_t(mt[4 * wi + q]) : 0u) << (8 * q);
+		dst[ref_words + wi] = word;
+	}
+	NvcMeshlet m;
+	memset(&m, 0, sizeof(m));
+	m.dataOffset = a.slot_data[s];
+	m.baseVertex = job.vertex_offset + lo;
+	m.vertexCount = uint8_t(r.z);
+	m.triangleCount = uint8_t(r.w);
+	m.shortRefs = short_refs ? 1 : 0;
+	cook::MeshletView view;
+	view.vertices = a.vertices;
+	view.data = dst;
+	view.baseVertex = m.baseVertex;
+	view.vertexCount = m.vertexCount;
+	view.triangleCount = m.triangleCount;
+	view.shortRefs = m.shortRefs;
+	cook::meshlet_bounds(view, &m);
+	a.meshlets[a.job_first[j] + local] = m;
+}
+
+} // namespace
+
+cudaError_t launch_cook_meshlets(const CookArgs& a, cudaStream_t stream)
+{
+	cudaError_t e = cudaMemsetAsync(a.totals4, 0, 16, stream);
+	if (e != cudaSuccess)
+		return e;
+	if (a.job_count)
+		cook_build_kernel<<<(a.job_count + kCookWarps - 1) / kCookWarps, kCookWarps * 32, 0, stream>>>(a);
+	if (a.slot_count)
+		cook_optimize_kernel<<<(a.slot_count + 127u) / 128u, 128, 0, stream>>>(a);
+	cook_scan_kernel<<<1, kCookScanThreads, 0, stream>>>(a);
+	if (a.slot_count)
+		cook_pack_kernel<<<(a.slot_count + 127u) / 128u, 128, 0, stream>>>(a);
 	return cudaGetLastError();
 }
 
