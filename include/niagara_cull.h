@@ -633,15 +633,41 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
  * meshletdata_capacity, totals4[3] is 1 and neither array is written (meshes is); nvc_cook_meshlets_capacity gives sizes
  * that always suffice.  NVC_ERROR_INVALID_ARGUMENT: lodCount > 8, an indexCount not a multiple of 3, or a LOD index range or
  * mesh vertex range outside indices / vertices.  Scratch is context-owned and grows as needed, and the call synchronises the
- * device before it enqueues its kernels on `stream`: call it at load time, outside stream capture.  Not covered: the
- * cooker's ray-tracing LOD of clrt builds (meshopt_buildMeshletsSpatial and meshletvtx0), the LOD chain itself
- * (meshopt_simplifyWithAttributes: the index ranges are inputs), and appending to existing Meshlet[] / meshletdata. */
+ * device before it enqueues its kernels on `stream`: call it at load time, outside stream capture.  The cooker of clrt
+ * builds (a ray-tracing LOD of spatial meshlets, meshletvtx0) is nvc_cook_meshlets_clrt below.  Not covered: the LOD chain
+ * itself (meshopt_simplifyWithAttributes: the index ranges are inputs), and appending to existing Meshlet[] / meshletdata. */
 NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices,
     uint32_t index_count, const NvcMesh* host_meshes, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity,
     uint32_t* meshletdata, uint32_t meshletdata_capacity, uint32_t* totals4);
 /* Host: capacities nvc_cook_meshlets never exceeds for these meshes: per LOD meshopt_buildMeshletsBound(indexCount, 64, 96)
  * meshlets and indexCount + ceil(indexCount / 4) + that bound words.  NVC_ERROR_INVALID_ARGUMENT when a lodCount > 8. */
 NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out);
+
+/* nvc_cook_meshlets as the reference's cooker runs in a clrt build (CLRT=1, niagara.cpp:844; scene.cpp:266-276, 52-67, 102-103),
+ * bit-identical to the Mesh[], Meshlet[], meshletdata and meshletvtx0 it stores:
+ *   max_scale    host, per mesh, the maxScale appendMesh receives: 1.0 for loadMesh, meshScale[i] for glTF (the mesh_scale
+ *                output of nvc_gltf_scene_arrays); NULL = 1.0 for every mesh
+ *   meshes       as nvc_cook_meshlets, and lodRT = the last LOD with lods[i].error * max_scale < 3e-3 (float multiply; 0 when
+ *                none is; NaN and inf fail the test); the input's lodRT is ignored
+ *   LOD lodRT    meshopt_buildMeshletsSpatial(64 vertices, min 24, max 96 triangles, fill weight 0.5) instead of the greedy
+ *                builder, then the same optimisation, packing and bounds; every other LOD exactly as nvc_cook_meshlets
+ *   meshletvtx0  device out: for each meshlet of each mesh's lodRT, in Meshlet[] order, per vertex (optimised order)
+ *                quantizeHalf(dequantizeHalf(v)) of x, y, z, then 0 (NaN becomes 0x7e00, fp16 denormals flush to 0);
+ *                may be NULL with capacity 0 (uint16 elements)
+ *   totals8      device out: meshlets needed, words needed, LODs rejected, overflow flag, meshletvtx0 elements needed
+ *                (counts saturated at 2^32 - 1), then three zeros
+ * A rejected lodRT (an index >= vertexCount) gets meshletCount 0 and contributes no meshletvtx0.  When any of the three
+ * capacities is exceeded, totals8[3] is 1 and none of the three arrays is written (meshes is).  Argument validation is
+ * nvc_cook_meshlets', plus meshletvtx0_capacity != 0 with meshletvtx0 NULL.  Scratch and synchronisation as nvc_cook_meshlets. */
+NVC_API int nvc_cook_meshlets_clrt(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices,
+    uint32_t index_count, const NvcMesh* host_meshes, const float* max_scale, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets,
+    uint32_t meshlet_capacity, uint32_t* meshletdata, uint32_t meshletdata_capacity, uint16_t* meshletvtx0, uint32_t meshletvtx0_capacity,
+    uint32_t* totals8);
+/* Host: capacities nvc_cook_meshlets_clrt never exceeds: nvc_cook_meshlets_capacity's per LOD, except that each mesh's lodRT
+ * takes meshopt_buildMeshletsBound(indexCount, 64, 24) meshlets (the array the reference sizes, scene.cpp:98), the matching
+ * words, and 4 * indexCount meshletvtx0 elements.  NVC_ERROR_INVALID_ARGUMENT when a lodCount > 8. */
+NVC_API int nvc_cook_meshlets_clrt_capacity(const NvcMesh* host_meshes, const float* max_scale, uint32_t mesh_count, uint32_t* meshlets_out,
+    uint64_t* words_out, uint64_t* vtx0_out);
 
 #ifdef __cplusplus
 } /* extern "C" */

@@ -751,6 +751,16 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_meshlet_bounds");
 }
 
+// scene.cpp:266-268: the last LOD with error * maxScale < kShadowLodError (0 when none is), with the reference's float multiply
+static uint32_t lod_rt(const NvcMesh& mesh, float max_scale)
+{
+	uint32_t rt = 0;
+	for (uint32_t i = 0; i < mesh.lodCount; ++i)
+		if (mesh.lods[i].error * max_scale < nvc::cook::kShadowLodError)
+			rt = i;
+	return rt;
+}
+
 NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out)
 {
 	if ((mesh_count && !host_meshes) || !meshlets_out || !words_out)
@@ -771,23 +781,34 @@ NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh
 	return NVC_OK;
 }
 
-NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices, uint32_t index_count,
+// nvc_cook_meshlets and, with clrt, nvc_cook_meshlets_clrt (whose meshletvtx0 arguments are unused otherwise)
+static int cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices, uint32_t index_count,
     const NvcMesh* host_meshes, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity, uint32_t* meshletdata,
-    uint32_t meshletdata_capacity, uint32_t* totals4)
+    uint32_t meshletdata_capacity, uint32_t* totals4, bool clrt, const float* max_scale, uint16_t* meshletvtx0, uint32_t meshletvtx0_capacity, const char* what)
 {
 	if (!ctx || !totals4 || (mesh_count && (!host_meshes || !meshes)) || (meshlet_capacity && !meshlets) || (meshletdata_capacity && !meshletdata))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (clrt && meshletvtx0_capacity && !meshletvtx0)
 		return NVC_ERROR_INVALID_ARGUMENT;
 	if (!device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 
 	// plan: one job per LOD in mesh then LOD order, each with its own scratch ranges
 	std::vector<nvc::cook::CookJob> jobs;
+	std::vector<uint32_t> job_rt;
+	// clrt: Mesh[] as uploaded, with lodRT set
+	std::vector<NvcMesh> rt_meshes;
+	if (clrt && mesh_count)
+		rt_meshes.assign(host_meshes, host_meshes + mesh_count);
 	uint64_t tri = 0, vtx = 0, idx = 0, slot = 0;
 	for (uint32_t i = 0; i < mesh_count; ++i)
 	{
 		const NvcMesh& mesh = host_meshes[i];
 		if (mesh.lodCount > NVC_MAX_LODS || uint64_t(mesh.vertexOffset) + mesh.vertexCount > vertex_count)
 			return NVC_ERROR_INVALID_ARGUMENT;
+		const uint32_t rt = clrt ? lod_rt(mesh, max_scale ? max_scale[i] : 1.0f) : NVC_MAX_LODS;
+		if (clrt)
+			rt_meshes[i].lodRT = rt;
 		for (uint32_t l = 0; l < mesh.lodCount; ++l)
 		{
 			const NvcMeshLod& lod = mesh.lods[l];
@@ -797,10 +818,11 @@ NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* ve
 				return NVC_ERROR_INVALID_ARGUMENT;
 			nvc::cook::CookJob job = { i, l, lod.indexOffset, lod.indexCount, mesh.vertexOffset, mesh.vertexCount, tri, vtx, idx, slot };
 			jobs.push_back(job);
+			job_rt.push_back(l == rt);
 			tri += lod.indexCount / 3;
 			vtx += mesh.vertexCount;
 			idx += lod.indexCount;
-			slot += nvc::cook::meshlets_bound(lod.indexCount);
+			slot += l == rt ? nvc::cook::spatial_meshlets_bound(lod.indexCount) : nvc::cook::meshlets_bound(lod.indexCount);
 		}
 	}
 	if (jobs.size() && !vertices)
@@ -808,11 +830,16 @@ NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* ve
 	if (slot > 0xffffffffull)
 		return NVC_ERROR_INVALID_ARGUMENT; // meshlet slots are counted in 32 bits
 	const uint32_t job_count = uint32_t(jobs.size());
-	// the longest jobs start first; outputs are placed by job index, so the order does not change them
+	// the longest jobs start first; outputs are placed by job index, so the order does not change them.  clrt: the greedy
+	// jobs, then the ray-tracing jobs, each longest first
 	std::vector<uint32_t> order(job_count);
 	for (uint32_t j = 0; j < job_count; ++j)
 		order[j] = j;
-	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+	auto longer = [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; };
+	auto rt_end = std::stable_partition(order.begin(), order.end(), [&](uint32_t x) { return !job_rt[x]; });
+	std::stable_sort(order.begin(), rt_end, longer);
+	std::stable_sort(rt_end, order.end(), longer);
+	const uint32_t greedy_count = uint32_t(rt_end - order.begin());
 
 	// scratch layout, 256-byte aligned sub-allocations
 	size_t bytes = 0;
@@ -827,6 +854,7 @@ NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* ve
 	size_t o_nodes = take(tri * 24u), o_kdi = take(tri * 4u), o_records = take(slot * 16u);
 	size_t o_words = take(slot * 4u), o_min = take(slot * 4u), o_sdata = take(slot * 4u);
 	size_t o_jm = take(job_count * 4ull), o_jf = take(job_count * 4ull);
+	size_t o_rt = take(clrt ? job_count * 4ull : 0), o_svtx = take(clrt ? slot * 4u : 0);
 
 	DeviceGuard guard(ctx->device);
 	// the previous call may still use the scratch, and the copies below are not ordered with `stream`
@@ -847,12 +875,14 @@ NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* ve
 		e = cudaMemcpy(base + o_jobs, jobs.data(), job_count * sizeof(nvc::cook::CookJob), cudaMemcpyHostToDevice);
 	if (e == cudaSuccess && job_count)
 		e = cudaMemcpy(base + o_order, order.data(), job_count * 4ull, cudaMemcpyHostToDevice);
+	if (e == cudaSuccess && clrt && job_count)
+		e = cudaMemcpy(base + o_rt, job_rt.data(), job_count * 4ull, cudaMemcpyHostToDevice);
 	if (e == cudaSuccess && mesh_count)
-		e = cudaMemcpy(meshes, host_meshes, size_t(mesh_count) * sizeof(NvcMesh), cudaMemcpyHostToDevice);
+		e = cudaMemcpy(meshes, clrt ? rt_meshes.data() : host_meshes, size_t(mesh_count) * sizeof(NvcMesh), cudaMemcpyHostToDevice);
 	if (e == cudaSuccess)
 		e = cudaDeviceSynchronize();
 	if (e != cudaSuccess)
-		return cuda_fail(ctx, e, "nvc_cook_meshlets");
+		return cuda_fail(ctx, e, what);
 
 	nvc::CookArgs a;
 	a.vertices = vertices;
@@ -883,8 +913,62 @@ NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* ve
 	a.meshletdata = meshletdata;
 	a.meshletdata_capacity = meshletdata_capacity;
 	a.totals4 = totals4;
-	e = nvc::launch_cook_meshlets(a, static_cast<cudaStream_t>(stream));
-	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_meshlets");
+	if (clrt)
+	{
+		nvc::CookClrtArgs c;
+		c.base = a;
+		c.greedy_count = greedy_count;
+		c.rt_count = job_count - greedy_count;
+		c.job_rt = reinterpret_cast<const uint32_t*>(base + o_rt);
+		c.slot_vtx0 = reinterpret_cast<uint32_t*>(base + o_svtx);
+		c.meshletvtx0 = meshletvtx0;
+		c.meshletvtx0_capacity = meshletvtx0_capacity;
+		e = nvc::launch_cook_meshlets_clrt(c, static_cast<cudaStream_t>(stream));
+	}
+	else
+		e = nvc::launch_cook_meshlets(a, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, what);
+}
+
+NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices, uint32_t index_count,
+    const NvcMesh* host_meshes, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity, uint32_t* meshletdata,
+    uint32_t meshletdata_capacity, uint32_t* totals4)
+{
+	return cook_meshlets(ctx, stream, vertices, vertex_count, indices, index_count, host_meshes, meshes, mesh_count, meshlets, meshlet_capacity, meshletdata,
+	    meshletdata_capacity, totals4, false, nullptr, nullptr, 0, "nvc_cook_meshlets");
+}
+
+NVC_API int nvc_cook_meshlets_clrt_capacity(const NvcMesh* host_meshes, const float* max_scale, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out,
+    uint64_t* vtx0_out)
+{
+	if ((mesh_count && !host_meshes) || !meshlets_out || !words_out || !vtx0_out)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	uint64_t meshlets = 0, words = 0, vtx0 = 0;
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		if (host_meshes[i].lodCount > NVC_MAX_LODS)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		const uint32_t rt = lod_rt(host_meshes[i], max_scale ? max_scale[i] : 1.0f);
+		for (uint32_t l = 0; l < host_meshes[i].lodCount; ++l)
+		{
+			const uint32_t n = host_meshes[i].lods[l].indexCount;
+			meshlets += l == rt ? nvc::cook::spatial_meshlets_bound(n) : nvc::cook::meshlets_bound(n);
+			words += l == rt ? nvc::cook::spatial_words_bound(n) : nvc::cook::words_bound(n);
+			vtx0 += l == rt ? 4ull * n : 0ull;
+		}
+	}
+	*meshlets_out = meshlets > 0xffffffffull ? 0xffffffffu : uint32_t(meshlets);
+	*words_out = words;
+	*vtx0_out = vtx0;
+	return NVC_OK;
+}
+
+NVC_API int nvc_cook_meshlets_clrt(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices, uint32_t index_count,
+    const NvcMesh* host_meshes, const float* max_scale, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity,
+    uint32_t* meshletdata, uint32_t meshletdata_capacity, uint16_t* meshletvtx0, uint32_t meshletvtx0_capacity, uint32_t* totals8)
+{
+	return cook_meshlets(ctx, stream, vertices, vertex_count, indices, index_count, host_meshes, meshes, mesh_count, meshlets, meshlet_capacity, meshletdata,
+	    meshletdata_capacity, totals8, true, max_scale, meshletvtx0, meshletvtx0_capacity, "nvc_cook_meshlets_clrt");
 }
 
 } // extern "C"

@@ -259,6 +259,19 @@ struct CookArgs
 	uint32_t* totals4;
 };
 cudaError_t launch_cook_meshlets(const CookArgs& a, cudaStream_t stream);
+// nvc_cook_meshlets_clrt: `base` as above, with base.order = the greedy jobs (largest first) followed by the ray-tracing
+// jobs (largest first), base.totals4 = totals8
+struct CookClrtArgs
+{
+	CookArgs base;
+	uint32_t greedy_count;  // base.order[0, greedy_count): meshopt_buildMeshlets jobs
+	uint32_t rt_count;      // base.order[greedy_count, + rt_count): meshopt_buildMeshletsSpatial jobs
+	const uint32_t* job_rt; // per job: 1 for the mesh's lodRT
+	uint32_t* slot_vtx0;    // per slot: first meshletvtx0 element
+	uint16_t* meshletvtx0;
+	uint32_t meshletvtx0_capacity;
+};
+cudaError_t launch_cook_meshlets_clrt(const CookClrtArgs& c, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);
 cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream);

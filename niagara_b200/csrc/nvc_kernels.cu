@@ -2917,7 +2917,469 @@ __global__ void __launch_bounds__(128) cook_pack_kernel(const CookArgs a)
 	a.meshlets[a.job_first[j] + local] = m;
 }
 
+// ---- clrt builds: meshopt_buildMeshletsSpatial for each mesh's lodRT (nvc_meshlets.cuh) ------------------------------------
+
+constexpr uint32_t kSpatialWarps = 4;          // jobs per block of the spatial build kernel
+constexpr uint32_t kSpatialStack = 64;         // pending bvhSplit nodes: at most depth + 2 <= kMaxTreeDepth + 2
+constexpr uint32_t kRadixBuckets = 1024;       // the reference's 10-bit digits
+
+// One LSD pass of the reference's radix sort (clusterizer.cpp:737-748): dst = src stably ordered by bits
+// [shift, shift + 10) of radixFloat(key).  hist is the warp's 1024 buckets.
+__device__ void spatial_radix_pass(uint32_t lane, uint32_t* dst, const uint32_t* src, const uint32_t* keys, uint32_t n, uint32_t shift, uint32_t* hist)
+{
+	const uint32_t full = 0xffffffffu;
+	for (uint32_t b = lane; b < kRadixBuckets; b += 32)
+		hist[b] = 0;
+	__syncwarp();
+	for (uint32_t i = lane; i < n; i += 32)
+	{
+		uint32_t u = keys[i];
+		atomicAdd(hist + (((u ^ ((uint32_t(int(u) >> 31)) | 0x80000000u)) >> shift) & 1023u), 1u);
+	}
+	__syncwarp();
+	// exclusive prefix: lane owns buckets [32 lane, 32 lane + 32)
+	uint32_t sum = 0;
+	for (uint32_t q = 0; q < 32; ++q)
+		sum += hist[lane * 32 + q];
+	uint32_t run = cook_warp_inclusive(sum, lane) - sum;
+	for (uint32_t q = 0; q < 32; ++q)
+	{
+		uint32_t c = hist[lane * 32 + q];
+		hist[lane * 32 + q] = run;
+		run += c;
+	}
+	__syncwarp();
+	// stable scatter, 32 elements at a time: rank among the earlier lanes of the same digit
+	for (uint32_t base = 0; base < n; base += 32)
+	{
+		uint32_t i = base + lane;
+		bool valid = i < n;
+		uint32_t v = valid ? src[i] : 0u, d = kRadixBuckets + lane;
+		if (valid)
+		{
+			uint32_t u = keys[v];
+			d = ((u ^ ((uint32_t(int(u) >> 31)) | 0x80000000u)) >> shift) & 1023u;
+		}
+		uint32_t peers = __match_any_sync(full, d);
+		uint32_t rank = __popc(peers & ((1u << lane) - 1u));
+		if (valid)
+			dst[hist[d] + rank] = v;
+		__syncwarp();
+		if (valid && (peers >> lane) == 1u) // the group's last lane moves the bucket on
+			hist[d] += __popc(peers);
+		__syncwarp();
+	}
+}
+
+// Inclusive running boxMerge component over the warp's 32 elements after `carry`.  box op NaN = NaN and NaN op x = x, so a
+// NaN element restarts the fold: the scan combines (value, restarted) pairs, which is associative.
+template <bool kMax>
+__device__ __forceinline__ float spatial_box_scan(float v, float carry, uint32_t lane)
+{
+	const uint32_t full = 0xffffffffu;
+	uint32_t r = v != v;
+	for (uint32_t d = 1; d < 32; d <<= 1)
+	{
+		float pv = __shfl_up_sync(full, v, d);
+		uint32_t pr = __shfl_up_sync(full, r, d);
+		if (lane >= d)
+		{
+			if (!r)
+				v = kMax ? cook::box_max(pv, v) : cook::box_min(pv, v);
+			r |= pr;
+		}
+	}
+	if (!r)
+		v = kMax ? cook::box_max(carry, v) : cook::box_min(carry, v);
+	return v;
+}
+
+// bvhComputeArea (clusterizer.cpp:866-878): areas[i] = area of boxes order[0..i], areas[count + i] = of order[count-1-i..]
+__device__ void spatial_areas(uint32_t lane, float* areas, const float* boxes, const uint32_t* order, uint32_t count)
+{
+	const uint32_t full = 0xffffffffu;
+	float lc[6] = { FLT_MAX, FLT_MAX, FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX };
+	float rc[6] = { FLT_MAX, FLT_MAX, FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX };
+	for (uint32_t base = 0; base < count; base += 32)
+	{
+		uint32_t i = base + lane;
+		bool valid = i < count;
+		uint32_t last = (count - base < 32 ? count - base : 32) - 1;
+		const float* lb = boxes + size_t(order[valid ? i : count - 1]) * 6u;
+		const float* rb = boxes + size_t(order[valid ? count - 1 - i : 0]) * 6u;
+		float l[6], r[6];
+		for (int k = 0; k < 3; ++k)
+		{
+			l[k] = spatial_box_scan<false>(lb[k], lc[k], lane);
+			l[k + 3] = spatial_box_scan<true>(lb[k + 3], lc[k + 3], lane);
+			r[k] = spatial_box_scan<false>(rb[k], rc[k], lane);
+			r[k + 3] = spatial_box_scan<true>(rb[k + 3], rc[k + 3], lane);
+		}
+		if (valid)
+		{
+			areas[i] = cook::box_area(l, l + 3);
+			areas[i + count] = cook::box_area(r, r + 3);
+		}
+		for (int k = 0; k < 6; ++k)
+		{
+			lc[k] = __shfl_sync(full, l[k], last);
+			rc[k] = __shfl_sync(full, r[k], last);
+		}
+	}
+}
+
+// bvhPivot by lanes.  bvhPivot keeps the first strict minimum of the full cost but skips candidates whose SAH part alone
+// exceeds the best so far.  A skipped candidate with full >= sah (the fill term >= 0) or full = NaN could not have won,
+// so where no candidate has full < sah the result is the first strict minimum of the full cost below FLT_MAX, reduced
+// over lanes by (cost, i).  Otherwise lane 0 runs the reference's loop as written.  The fill term is negative only when the
+// float round-up int(float(fill + maxfill - 1) * (1.f / maxfill)) truncates low, which it does not for any fill below 2^25 with
+// maxfill 64 or 96 (checked exhaustively in float32), so the fallback only guards LODs of 2^25 triangles and more.
+__device__ uint32_t spatial_pivot(uint32_t lane, const float* areas, const uint32_t* vertices, uint32_t count, uint32_t min, uint32_t maxfill, float& out_cost)
+{
+	const uint32_t full_mask = 0xffffffffu;
+	bool aligned = cook::pivot_aligned(count, min);
+	uint32_t end = cook::pivot_end(count, min);
+	float rmaxfill = cook::div(1.0f, float(int(maxfill)));
+	uint32_t bkey = 0xffffffffu, bi = 0xffffffffu, bbits = 0;
+	bool skip_matters = false;
+	for (uint32_t i = min - 1 + lane; i < end; i += 32)
+	{
+		float sah, full;
+		if (!cook::pivot_cost(areas, vertices, count, i, min, aligned, maxfill, rmaxfill, sah, full))
+			continue;
+		skip_matters = skip_matters || full < sah;
+		if (!(full < FLT_MAX))
+			continue;
+		uint32_t key = cook_score_key(full);
+		if (key < bkey) // i increases within a lane: the first of equal costs is kept
+		{
+			bkey = key;
+			bi = i;
+			bbits = cook::float_bits(full);
+		}
+	}
+	for (int d = 16; d > 0; d >>= 1)
+	{
+		uint32_t ok = __shfl_xor_sync(full_mask, bkey, d), oi = __shfl_xor_sync(full_mask, bi, d), ob = __shfl_xor_sync(full_mask, bbits, d);
+		if (ok < bkey || (ok == bkey && oi < bi))
+			bkey = ok, bi = oi, bbits = ob;
+	}
+	if (__any_sync(full_mask, skip_matters))
+	{
+		uint32_t split = 0;
+		float cost = FLT_MAX;
+		if (lane == 0)
+			split = cook::bvh_pivot(areas, vertices, count, min, maxfill, cost);
+		out_cost = __shfl_sync(full_mask, cost, 0);
+		return __shfl_sync(full_mask, split, 0);
+	}
+	out_cost = bi == 0xffffffffu ? FLT_MAX : cook::bits_float(bbits);
+	return bi == 0xffffffffu ? 0u : bi + 1;
+}
+
+// One warp per ray-tracing job: meshopt_buildMeshletsSpatial (clusterizer.cpp:1266-1365) with the parameters of
+// scene.cpp:103.  Fills the same per-job outputs as cook_build_kernel (records in the job's slots, ml_vertices,
+// ml_triangles, job_meshlets); the optimize, scan and pack kernels then treat both kinds of job alike.  Scratch of the job
+// (sized for the greedy builder): cones = boxes (6 floats per triangle), kd_nodes = the three axis orders then the sort
+// keys / areas, kd_index = sort and partition temp, emitted = sides, adj_data = boundary bytes.  bvhSplit's recursion
+// is a depth-first stack of (start, count, depth); each node's work is spread over the lanes.
+__global__ void __launch_bounds__(kSpatialWarps * 32) cook_spatial_kernel(const CookClrtArgs c)
+{
+	__shared__ uint32_t s_hist[kSpatialWarps][kRadixBuckets];
+	const CookArgs& a = c.base;
+	const uint32_t full = 0xffffffffu;
+	const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+	const uint32_t w = blockIdx.x * kSpatialWarps + warp;
+	if (w >= c.rt_count)
+		return;
+	const uint32_t j = a.order[c.greedy_count + w];
+	const cook::CookJob job = a.jobs[j];
+	const uint32_t* indices = a.indices + job.index_offset;
+	const uint32_t index_count = job.index_count, n = index_count / 3, vertex_count = job.vertex_count;
+
+	bool bad = false;
+	for (uint32_t i = lane; i < index_count; i += 32)
+		bad = bad || indices[i] >= vertex_count;
+	if (__any_sync(full, bad) || n == 0)
+	{
+		if (lane == 0)
+		{
+			a.job_meshlets[j] = 0;
+			if (n != 0)
+				atomicAdd(a.totals4 + 2, 1u);
+		}
+		return;
+	}
+
+	float* boxes = a.cones + job.tri * 6u;
+	uint32_t* axes = a.kd_nodes + job.tri * 6u;
+	uint32_t* keys = axes + 3u * n;
+	float* areas = reinterpret_cast<float*>(keys);
+	uint32_t* temp = a.kd_index + job.tri;
+	uint8_t* sides = a.emitted + job.tri;
+	uint8_t* boundary = reinterpret_cast<uint8_t*>(a.adj_data + job.idx);
+	int16_t* used = a.used + job.vtx;
+	uint32_t* mlv = a.ml_vertices + job.idx;
+	uint8_t* mlt = a.ml_triangles + job.idx;
+	uint4* records = a.ml_records + job.slot;
+	const NvcVertex* verts = a.vertices + job.vertex_offset;
+
+	// bvhPrepare (clusterizer.cpp:750-775)
+	for (uint32_t t = lane; t < n; t += 32)
+	{
+		float p[3][3];
+		for (int q = 0; q < 3; ++q)
+		{
+			const NvcVertex& v = verts[indices[t * 3 + q]];
+			p[q][0] = cook::dequantize_half(v.vx);
+			p[q][1] = cook::dequantize_half(v.vy);
+			p[q][2] = cook::dequantize_half(v.vz);
+		}
+		for (int k = 0; k < 3; ++k)
+		{
+			float mn = p[0][k] < p[1][k] ? p[0][k] : p[1][k];
+			mn = p[2][k] < mn ? p[2][k] : mn;
+			float mx = p[0][k] > p[1][k] ? p[0][k] : p[1][k];
+			mx = p[2][k] > mx ? p[2][k] : mx;
+			boxes[size_t(t) * 6u + k] = mn;
+			boxes[size_t(t) * 6u + 3 + k] = mx;
+			keys[k * n + t] = cook::float_bits(cook::centroid(mn, mx));
+		}
+	}
+	for (uint32_t v = lane; v < vertex_count; v += 32)
+		used[v] = -1;
+	__syncwarp();
+
+	// the three radix sorts (clusterizer.cpp:1300-1314), from identity order
+	for (int k = 0; k < 3; ++k)
+	{
+		uint32_t* order = axes + k * n;
+		for (uint32_t i = lane; i < n; i += 32)
+			temp[i] = i;
+		__syncwarp();
+		spatial_radix_pass(lane, order, temp, keys + k * n, n, 2, s_hist[warp]);
+		spatial_radix_pass(lane, temp, order, keys + k * n, n, 12, s_hist[warp]);
+		spatial_radix_pass(lane, order, temp, keys + k * n, n, 22, s_hist[warp]);
+	}
+	__syncwarp();
+
+	// bvhSplit (clusterizer.cpp:942-1012)
+	uint32_t st_start[kSpatialStack], st_count[kSpatialStack];
+	int st_depth[kSpatialStack];
+	int sp = 0;
+	st_start[0] = 0, st_count[0] = n, st_depth[0] = 0, sp = 1;
+	while (sp > 0)
+	{
+		--sp;
+		const uint32_t start = st_start[sp], count = st_count[sp];
+		const int depth = st_depth[sp];
+		uint8_t* bnd = boundary + start;
+		if (count <= cook::kMaxTriangles)
+		{
+			uint32_t nv = 0;
+			if (lane == 0)
+				nv = cook::bvh_count_vertices(axes + start, count, used, indices, nullptr);
+			nv = __shfl_sync(full, nv, 0);
+			if (nv <= cook::kMaxVertices)
+			{
+				for (uint32_t i = lane; i < count; i += 32)
+					bnd[i] = i == 0;
+				__syncwarp();
+				continue;
+			}
+		}
+		// a node of <= 96 triangles that did not pack is vertex bound
+		const uint32_t mint = count <= cook::kMaxTriangles ? cook::kSpatialLeafSplit : cook::kSpatialMinTriangles;
+		const uint32_t maxfill = count <= cook::kMaxTriangles ? cook::kMaxVertices : cook::kMaxTriangles;
+		int bestk = -1;
+		uint32_t bestsplit = 0;
+		float bestcost = FLT_MAX;
+		for (int k = 0; k < 3; ++k)
+		{
+			const uint32_t* order = axes + k * n + start;
+			spatial_areas(lane, areas, boxes, order, count);
+			uint32_t* vertices = nullptr;
+			if (count <= cook::kMaxTriangles)
+			{
+				vertices = reinterpret_cast<uint32_t*>(areas + 2 * count);
+				if (lane == 0)
+					cook::bvh_count_vertices(order, count, used, indices, vertices);
+			}
+			__syncwarp();
+			float axiscost = FLT_MAX;
+			uint32_t axissplit = spatial_pivot(lane, areas, vertices, count, mint, maxfill, axiscost);
+			if (axissplit && axiscost < bestcost)
+			{
+				bestk = k;
+				bestcost = axiscost;
+				bestsplit = axissplit;
+			}
+			__syncwarp();
+		}
+		if (bestk < 0 || depth >= cook::kMaxTreeDepth)
+		{
+			if (lane == 0)
+				cook::bvh_pack_tail(bnd, axes + start, count, used, indices);
+			__syncwarp();
+			continue;
+		}
+		const uint32_t* best = axes + bestk * n + start;
+		for (uint32_t i = lane; i < count; i += 32)
+			sides[best[i]] = i >= bestsplit;
+		__syncwarp();
+		// bvhPartition of the two other axes (clusterizer.cpp:928-940), stable, 32 elements at a time
+		for (int k = 0; k < 3; ++k)
+		{
+			if (k == bestk)
+				continue;
+			uint32_t* axis = axes + k * n + start;
+			for (uint32_t i = lane; i < count; i += 32)
+				temp[i] = axis[i];
+			__syncwarp();
+			uint32_t l = 0, r = bestsplit;
+			for (uint32_t base = 0; base < count; base += 32)
+			{
+				uint32_t i = base + lane;
+				bool valid = i < count;
+				uint32_t v = valid ? temp[i] : 0u;
+				bool side = valid && sides[v];
+				uint32_t lm = __ballot_sync(full, valid && !side), rm = __ballot_sync(full, side);
+				uint32_t below = (1u << lane) - 1u;
+				if (valid)
+					axis[side ? r + __popc(rm & below) : l + __popc(lm & below)] = v;
+				l += __popc(lm);
+				r += __popc(rm);
+			}
+			__syncwarp();
+		}
+		st_start[sp] = start + bestsplit, st_count[sp] = count - bestsplit, st_depth[sp] = depth + 1, ++sp;
+		st_start[sp] = start, st_count[sp] = bestsplit, st_depth[sp] = depth + 1, ++sp;
+	}
+
+	// the packing loop (clusterizer.cpp:1326-1358), sequential: boundaries, the over-bound rule and appendMeshlet's own splits
+	uint32_t marks = 0;
+	for (uint32_t i = lane; i < n; i += 32)
+		marks += boundary[i];
+	const uint32_t meshlet_count = __shfl_sync(full, cook_warp_inclusive(marks, lane), 31);
+	if (lane == 0)
+	{
+		const uint64_t meshlet_bound = cook::spatial_meshlets_bound(index_count);
+		cook::Building m = { 0, 0, 0, 0 };
+		uint64_t meshlet_offset = 0, meshlet_pending = meshlet_count;
+		bool over = false;
+		for (uint32_t i = 0; i < n; ++i)
+		{
+			bool split = i > 0 && boundary[i] == 1;
+			if (split && meshlet_count > meshlet_bound && meshlet_offset + meshlet_pending >= meshlet_bound)
+				split = false;
+			// the reference asserts meshlet_offset <= meshlet_bound; the job's slots end there
+			if (meshlet_offset >= meshlet_bound)
+			{
+				over = true;
+				break;
+			}
+			// appendMeshlet(..., split): a split flushes first, and the emptied meshlet then takes the triangle without a flush
+			uint32_t index = axes[i];
+			if (split)
+				cook::flush_meshlet(m, used, records, uint32_t(meshlet_offset), mlv);
+			bool flushed = cook::append_triangle(m, indices[index * 3 + 0], indices[index * 3 + 1], indices[index * 3 + 2], used, records, uint32_t(meshlet_offset), mlv, mlt);
+			meshlet_offset += (split || flushed) ? 1u : 0u;
+			meshlet_pending -= boundary[i];
+		}
+		if (!over && m.triangle_count)
+		{
+			if (meshlet_offset >= meshlet_bound)
+				over = true;
+			else
+				records[meshlet_offset++] = make_uint4(m.vertex_offset, m.triangle_offset, m.vertex_count, m.triangle_count);
+		}
+		a.job_meshlets[j] = over ? 0u : uint32_t(meshlet_offset);
+		if (over)
+			atomicAdd(a.totals4 + 2, 1u);
+	}
+}
+
+// meshletvtx0 offsets (scene.cpp:52-67): 4 elements per vertex of every meshlet of a ray-tracing job, in slot order (= job,
+// then meshlet order); totals8[4] and the overflow flag.  Runs after cook_scan_kernel, before the pack kernels.
+__global__ void __launch_bounds__(kCookScanThreads) cook_vtx0_scan_kernel(const CookClrtArgs c)
+{
+	__shared__ uint32_t s_warp[32];
+	const CookArgs& a = c.base;
+	uint64_t carry = 0;
+	for (uint32_t base = 0; base < a.slot_count; base += kCookScanThreads)
+	{
+		uint32_t s = base + threadIdx.x, n = 0, total;
+		if (s < a.slot_count)
+		{
+			uint32_t j = cook_job_of_slot(a, s);
+			if (c.job_rt[j] && s - uint32_t(a.jobs[j].slot) < a.job_meshlets[j])
+				n = 4u * a.ml_records[s].z;
+		}
+		uint32_t before = cook_block_exclusive(n, total, s_warp);
+		if (s < a.slot_count)
+			c.slot_vtx0[s] = uint32_t(carry + before);
+		carry += total;
+	}
+	if (threadIdx.x == 0)
+	{
+		a.totals4[4] = carry > 0xffffffffull ? 0xffffffffu : uint32_t(carry);
+		if (carry > c.meshletvtx0_capacity)
+			a.totals4[3] = 1u;
+	}
+}
+
+// One thread per ray-tracing meshlet: quantizeHalf of its positions (the dequantized fp16 of Vertex, so NaN becomes
+// 0x7e00 and denormals flush to 0) in the optimized vertex order, then 0.  Nothing is written on overflow.
+__global__ void __launch_bounds__(128) cook_vtx0_pack_kernel(const CookClrtArgs c)
+{
+	const CookArgs& a = c.base;
+	uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+	if (s >= a.slot_count || a.totals4[3])
+		return;
+	uint32_t j = cook_job_of_slot(a, s);
+	const cook::CookJob& job = a.jobs[j];
+	if (!c.job_rt[j] || s - uint32_t(job.slot) >= a.job_meshlets[j])
+		return;
+	uint4 r = a.ml_records[s];
+	const uint32_t* mv = a.ml_vertices + job.idx + r.x;
+	uint16_t* dst = c.meshletvtx0 + c.slot_vtx0[s];
+	for (uint32_t i = 0; i < r.z; ++i)
+	{
+		const NvcVertex& v = a.vertices[job.vertex_offset + mv[i]];
+		dst[4 * i + 0] = cook::quantize_half(cook::dequantize_half(v.vx));
+		dst[4 * i + 1] = cook::quantize_half(cook::dequantize_half(v.vy));
+		dst[4 * i + 2] = cook::quantize_half(cook::dequantize_half(v.vz));
+		dst[4 * i + 3] = 0;
+	}
+}
+
 } // namespace
+
+cudaError_t launch_cook_meshlets_clrt(const CookClrtArgs& c, cudaStream_t stream)
+{
+	const CookArgs& a = c.base;
+	cudaError_t e = cudaMemsetAsync(a.totals4, 0, 32, stream);
+	if (e != cudaSuccess)
+		return e;
+	if (c.greedy_count)
+	{
+		CookArgs g = a;
+		g.job_count = c.greedy_count; // the build kernel takes order[0, job_count)
+		cook_build_kernel<<<(c.greedy_count + kCookWarps - 1) / kCookWarps, kCookWarps * 32, 0, stream>>>(g);
+	}
+	if (c.rt_count)
+		cook_spatial_kernel<<<(c.rt_count + kSpatialWarps - 1) / kSpatialWarps, kSpatialWarps * 32, 0, stream>>>(c);
+	if (a.slot_count)
+		cook_optimize_kernel<<<(a.slot_count + 127u) / 128u, 128, 0, stream>>>(a);
+	cook_scan_kernel<<<1, kCookScanThreads, 0, stream>>>(a);
+	cook_vtx0_scan_kernel<<<1, kCookScanThreads, 0, stream>>>(c);
+	if (a.slot_count)
+	{
+		cook_pack_kernel<<<(a.slot_count + 127u) / 128u, 128, 0, stream>>>(a);
+		cook_vtx0_pack_kernel<<<(a.slot_count + 127u) / 128u, 128, 0, stream>>>(c);
+	}
+	return cudaGetLastError();
+}
 
 cudaError_t launch_cook_meshlets(const CookArgs& a, cudaStream_t stream)
 {

@@ -425,5 +425,164 @@ NVC_HD void optimize_meshlet(uint32_t* vertices, uint32_t vertex_count, uint8_t*
 		vertices[i] = order[i];
 }
 
+// ---- clrt builds: the ray-tracing LOD (scene.cpp:102-103) -----------------------------------------------------------------
+// meshopt_buildMeshletsSpatial(max_vertices 64, min_triangles 24, max_triangles 96, fill_weight 0.5), clusterizer.cpp:640-1013,
+// 1266-1365, as compiled for x86-64 (SIMD_SSE).  The sort, the box scans, the pivot search and the partitions are warp-parallel
+// in the kernel (nvc_kernels.cu); what is sequential there is spelled here.  Since min_triangles != max_triangles, bvhSplit's
+// pivot step is always 1.
+
+constexpr uint32_t kSpatialMinTriangles = kMaxTriangles / 4; // MESH_MAXTRI / 4 (scene.cpp:93)
+constexpr float kFillWeight = 0.5f;                           // MESHLET_FILL_WEIGHT (config.h)
+constexpr float kShadowLodError = 3e-3f;                      // scene.cpp:22, the lodRT threshold
+constexpr uint32_t kSpatialLeafSplit = kMaxVertices / 3;      // bvhPackTail's chunk of a vertex-bound run, and bvhSplit's mint
+
+// meshopt_buildMeshletsBound(index_count, 64, 24): the meshlet array the reference sizes for every LOD (scene.cpp:98)
+NVC_HD uint64_t spatial_meshlets_bound(uint64_t index_count)
+{
+	uint64_t by_vertices = (index_count + (kMaxVertices - 2) - 1) / (kMaxVertices - 2);
+	uint64_t by_triangles = (index_count / 3 + kSpatialMinTriangles - 1) / kSpatialMinTriangles;
+	return by_vertices > by_triangles ? by_vertices : by_triangles;
+}
+
+// as words_bound, with the spatial meshlet bound
+NVC_HD uint64_t spatial_words_bound(uint64_t index_count) { return index_count + (index_count + 3) / 4 + spatial_meshlets_bound(index_count); }
+
+// the SSE boxMerge per component: _mm_min_ps / _mm_max_ps return the second operand (the merged box) on ties and NaN
+NVC_HD float box_min(float box, float other) { return box < other ? box : other; }
+NVC_HD float box_max(float box, float other) { return box > other ? box : other; }
+
+// bvhPrepare's centroid (min + max) / 2.f with the NaN bits of x86 SSE, the reference's target: a NaN operand comes back
+// quieted (the first one when both are NaN) and a NaN made from numbers (inf - inf) is the default NaN 0xffc00000.  The GPU's
+// arithmetic returns 0x7fffffff for both.  The radix sort orders NaN centroids by these bits.
+NVC_HD float centroid(float mn, float mx)
+{
+	if (mn != mn)
+		return bits_float(float_bits(mn) | 0x00400000u);
+	if (mx != mx)
+		return bits_float(float_bits(mx) | 0x00400000u);
+	float s = add(mn, mx);
+	return s != s ? bits_float(0xffc00000u) : div(s, 2.0f);
+}
+
+// the SSE boxMerge's area: (sx * sy + sy * sz) + sz * sx
+NVC_HD float box_area(const float mn[3], const float mx[3])
+{
+	float sx = sub(mx[0], mn[0]), sy = sub(mx[1], mn[1]), sz = sub(mx[2], mn[2]);
+	return add(add(mul(sx, sy), mul(sy, sz)), mul(sz, sx));
+}
+
+// bvhCountVertices (clusterizer.cpp:816-840): unique vertices of order[0..count), out[i] after triangle i when out is given
+// (a triangle with a repeated new vertex counts it twice, as in the reference); used[] is left all -1
+NVC_HD uint32_t bvh_count_vertices(const uint32_t* order, uint32_t count, int16_t* used, const uint32_t* indices, uint32_t* out)
+{
+	uint32_t used_vertices = 0;
+	for (uint32_t i = 0; i < count; ++i)
+	{
+		uint32_t index = order[i];
+		uint32_t a = indices[index * 3 + 0], b = indices[index * 3 + 1], c = indices[index * 3 + 2];
+		used_vertices += (used[a] < 0) + (used[b] < 0) + (used[c] < 0);
+		used[a] = used[b] = used[c] = 1;
+		if (out)
+			out[i] = used_vertices;
+	}
+	for (uint32_t i = 0; i < count; ++i)
+	{
+		uint32_t index = order[i];
+		used[indices[index * 3 + 0]] = used[indices[index * 3 + 1]] = used[indices[index * 3 + 2]] = -1;
+	}
+	return used_vertices;
+}
+
+NVC_HD void bvh_pack_leaf(uint8_t* boundary, uint32_t count)
+{
+	boundary[0] = 1;
+	for (uint32_t i = 1; i < count; ++i)
+		boundary[i] = 0;
+}
+
+// bvhPackTail (clusterizer.cpp:851-870)
+NVC_HD void bvh_pack_tail(uint8_t* boundary, const uint32_t* order, uint32_t count, int16_t* used, const uint32_t* indices)
+{
+	for (uint32_t i = 0; i < count;)
+	{
+		uint32_t chunk = i + kMaxTriangles <= count ? kMaxTriangles : count - i;
+		if (bvh_count_vertices(order + i, chunk, used, indices, nullptr) <= kMaxVertices)
+		{
+			bvh_pack_leaf(boundary + i, chunk);
+			i += chunk;
+			continue;
+		}
+		bvh_pack_leaf(boundary + i, kSpatialLeafSplit);
+		i += kSpatialLeafSplit;
+	}
+}
+
+// bvhDivisible (clusterizer.cpp:872-878)
+NVC_HD bool bvh_divisible(uint32_t count, uint32_t min, uint32_t max)
+{
+	return min * 2 <= max ? count >= min : count % min <= (count / min) * (max - min);
+}
+
+// One candidate i of bvhPivot (clusterizer.cpp:895-920): false if not admissible; else `sah`, the cost the early
+// `cost > bestcost` skip tests, and `full`, the cost with the fill term.  rfill is the left count, as written.
+NVC_HD bool pivot_cost(const float* areas, const uint32_t* vertices, uint32_t count, uint32_t i, uint32_t min, bool aligned, uint32_t maxfill,
+    float rmaxfill, float& sah, float& full)
+{
+	uint32_t lsplit = i + 1, rsplit = count - (i + 1);
+	if (!bvh_divisible(lsplit, min, kMaxTriangles))
+		return false;
+	if (aligned && !bvh_divisible(rsplit, min, kMaxTriangles))
+		return false;
+	float larea = areas[i], rarea = areas[(count - 1 - (i + 1)) + count];
+	sah = add(mul(larea, float(int(lsplit))), mul(rarea, float(int(rsplit))));
+	uint32_t lfill = vertices ? vertices[i] : lsplit;
+	uint32_t rfill = vertices ? vertices[i] : rsplit;
+	int lrest = int(mul(float(int(lfill + maxfill - 1)), rmaxfill)) * int(maxfill) - int(lfill);
+	int rrest = int(mul(float(int(rfill + maxfill - 1)), rmaxfill)) * int(maxfill) - int(rfill);
+	full = add(sah, mul(kFillWeight, add(mul(float(lrest), larea), mul(float(rrest), rarea))));
+	return true;
+}
+
+// bvhPivot's admissible range: [min - 1, end)
+NVC_HD bool pivot_aligned(uint32_t count, uint32_t min) { return count >= min * 2 && bvh_divisible(count, min, kMaxTriangles); }
+NVC_HD uint32_t pivot_end(uint32_t count, uint32_t min) { return pivot_aligned(count, min) ? count - min : count - 1; }
+
+// bvhPivot (clusterizer.cpp:880-926) as written, with its early skip: the split after the first strict minimum
+NVC_HD uint32_t bvh_pivot(const float* areas, const uint32_t* vertices, uint32_t count, uint32_t min, uint32_t maxfill, float& out_cost)
+{
+	bool aligned = pivot_aligned(count, min);
+	uint32_t end = pivot_end(count, min);
+	float rmaxfill = div(1.0f, float(int(maxfill)));
+	uint32_t bestsplit = 0;
+	float bestcost = FLT_MAX;
+	for (uint32_t i = min - 1; i < end; ++i)
+	{
+		float sah, full;
+		if (!pivot_cost(areas, vertices, count, i, min, aligned, maxfill, rmaxfill, sah, full))
+			continue;
+		if (sah > bestcost)
+			continue;
+		if (full < bestcost)
+		{
+			bestcost = full;
+			bestsplit = i + 1;
+		}
+	}
+	out_cost = bestcost;
+	return bestsplit;
+}
+
+// appendMeshlet's flush (clusterizer.cpp:262-275), for the spatial packing loop's `split`
+NVC_HD void flush_meshlet(Building& m, int16_t* used, uint4* records, uint32_t meshlet_offset, const uint32_t* meshlet_vertices)
+{
+	records[meshlet_offset] = make_uint4(m.vertex_offset, m.triangle_offset, m.vertex_count, m.triangle_count);
+	for (uint32_t j = 0; j < m.vertex_count; ++j)
+		used[meshlet_vertices[m.vertex_offset + j]] = -1;
+	m.vertex_offset += m.vertex_count;
+	m.triangle_offset += m.triangle_count * 3;
+	m.vertex_count = 0;
+	m.triangle_count = 0;
+}
+
 } // namespace cook
 } // namespace nvc
