@@ -250,6 +250,8 @@ NVC_API void nvc_destroy(NvcContext* ctx)
 		cudaFree(ctx->hiz_fp);
 	if (ctx->cook_scratch)
 		cudaFree(ctx->cook_scratch);
+	if (ctx->cache_scratch)
+		cudaFree(ctx->cache_scratch);
 	delete ctx;
 }
 

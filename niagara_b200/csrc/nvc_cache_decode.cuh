@@ -1,0 +1,369 @@
+// nvc_cache_decode.cuh — device decoders of a compressed scene cache's vertex and meshlet streams, for
+// nvc_scene_cache_read_device (nvc_scene_cache_device.cpp).  Their outputs equal the host decoders'
+// (nvc_meshopt_decode.cpp, nvc_scene_cache.cpp) byte for byte; the formats are restated there.
+//
+// Vertex codec (VERTICES, stride 16; MESHLETVTX0, stride 8).  The host walk (walk_vertex_stream) has already checked the
+// whole stream and found every block's and every byte plane's start, so nothing here can fail.  Three launches:
+//   blocks   one warp per block of 256 vertices: stage the block's bytes in shared memory; one lane per plane finds its
+//            groups' offsets from the selectors and the escape counts (nvc_meshopt_format.h); one lane per (plane, group)
+//            unpacks; then per 4-byte column a warp scan of the delta terms with the previous vertex taken as 0.  The
+//            block's words go out coalesced; its last vertex's words are the block's totals.
+//   carry    one CTA per column: exclusive scan of the block totals from the baseline vertex (the column's channel fixes
+//            the combination for the whole stream, and each is an abelian group, so the scan is exact).
+//   apply    every output word combined with its block's carry.
+// Meshlet codec (MESHLETDATA).  Each block is a serial chain (triangle history, unseen counter, explicit-byte cursor), so
+// one lane decodes one meshlet.  A warp takes the 32 meshlets after one checkpoint of the host's index: their blocks are
+// adjacent in the stream and are staged in shared memory as one coalesced span when it fits (the reference's 64 / 96
+// meshlets take about 5 KB), else read where they lie.  Every read is bounded by the block's own extent from the size
+// chain, exactly as the host decoder bounds it; a malformed block raises a flag (NVC_ERROR_CORRUPT).  Outputs are whole
+// words: the host index admits only caches whose meshlets' word ranges do not overlap, so a meshlet owns its words, and
+// the zero bytes a word holds past the meshlet's last reference or triangle are what the host's zero fill leaves there.
+#pragma once
+
+#include "nvc_internal.h"
+#include "nvc_meshopt_format.h"
+
+namespace nvc
+{
+namespace cache
+{
+
+constexpr uint32_t kVertexBlock = 256; // vcodec::block_vertices of strides 8 and 16
+constexpr uint32_t kVertexWarps = 4;
+constexpr uint32_t kCarryThreads = 1024;
+constexpr uint32_t kApplyThreads = 256;
+constexpr uint32_t kMeshletWarps = 4;
+constexpr uint32_t kMeshletStageWords = 2048; // 8 KB per warp
+
+// Shared memory of one warp of the block kernel.  span: the most bytes one block of stride S can span (its control bytes,
+// then per plane the selector header and 16 groups of at most 24 bytes: 4-bit fields that are all escaped).  words: that
+// span staged from a word boundary; later the block's decoded words, padded by one word per 8 vertices so that the lanes'
+// stores (8 consecutive vertices each) fall into distinct banks.
+template <uint32_t S>
+struct VertexStage
+{
+	static constexpr uint32_t span = S / 4 + S * (4 + 16 * 24);
+	static constexpr uint32_t staged = (span + 3 + 3) / 4, decoded = kVertexBlock * S / 4 + 32;
+	static constexpr uint32_t words = staged > decoded ? staged : decoded;
+};
+
+// v[k] by selects: a dynamic index into a kernel parameter array would copy the array to the stack
+__device__ __forceinline__ uint32_t column_value(const uint32_t (&v)[4], uint32_t k)
+{
+	return k == 0 ? v[0] : k == 1 ? v[1] : k == 2 ? v[2] : v[3];
+}
+
+__device__ __forceinline__ uint32_t padded_word(uint32_t vertex, uint32_t column, uint32_t columns)
+{
+	return vertex * columns + column + vertex / 8u;
+}
+
+template <uint32_t S>
+__global__ void __launch_bounds__(kVertexWarps * 32) decode_vertex_blocks_kernel(const VertexDecodeArgs a)
+{
+	constexpr uint32_t C = S / 4;
+	const uint32_t full = 0xffffffffu;
+	__shared__ uint32_t s_stage[kVertexWarps][VertexStage<S>::words];
+	__shared__ __align__(8) uint8_t s_planes[kVertexWarps][S * kVertexBlock];
+	__shared__ uint16_t s_group[kVertexWarps][S * 16];
+	__shared__ uint16_t s_plane[kVertexWarps][S];
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	const uint32_t b = blockIdx.x * kVertexWarps + warp;
+	if (b >= a.blocks)
+		return; // whole warps
+	const uint32_t first = b * kVertexBlock;
+	const uint32_t n = min(a.vertex_count - first, kVertexBlock), groups = (n + 15u) / 16u;
+	uint32_t* stage = s_stage[warp];
+	uint8_t* planes = s_planes[warp];
+	uint16_t* group = s_group[warp];
+
+	const uint32_t start = a.block_start[b], end = a.block_start[b + 1];
+	const uint32_t* src = reinterpret_cast<const uint32_t*>(a.stream) + start / 4u;
+	const uint32_t words = end / 4u + ((end & 3u) != 0) - start / 4u; // no wrap for offsets near 2^32
+	for (uint32_t i = lane; i < words; i += 32)
+		stage[i] = __ldg(src + i);
+	__syncwarp();
+	const uint8_t* block = reinterpret_cast<const uint8_t*>(stage) + (start & 3u);
+
+	// each plane's control (v1: 2 bits per plane in the block's leading bytes) and its groups' offsets in the block
+	if (lane < S)
+	{
+		const uint32_t p0 = a.plane_offset[size_t(b) * S + lane];
+		s_plane[warp][lane] = uint16_t(p0);
+		const int control = a.version ? int((block[lane / 4] >> ((lane % 4) * 2)) & 3u) : 0;
+		if (control < 2)
+		{
+			uint32_t at = p0 + vcodec::selector_bytes(groups);
+			for (uint32_t g = 0; g < groups; ++g)
+			{
+				group[lane * 16 + g] = uint16_t(at);
+				at += vcodec::group_bytes(block + at, vcodec::group_width(a.version, control, (block[p0 + g / 4] >> ((g % 4) * 2)) & 3u));
+			}
+		}
+	}
+	__syncwarp();
+
+	// unpack: one lane per (plane, group of 16 values)
+	for (uint32_t item = lane; item < S * 16; item += 32)
+	{
+		const uint32_t q = item >> 4, g = item & 15u;
+		if (g >= groups)
+			continue;
+		const uint32_t p0 = s_plane[warp][q];
+		const int control = a.version ? int((block[q / 4] >> ((q % 4) * 2)) & 3u) : 0;
+		uint8_t* out = planes + q * kVertexBlock + g * 16;
+		if (control == 3)
+			for (uint32_t i = 0; i < 16; ++i)
+				out[i] = g * 16 + i < n ? block[p0 + g * 16 + i] : 0;
+		else if (control == 2)
+			for (uint32_t i = 0; i < 16; ++i)
+				out[i] = 0;
+		else
+		{
+			const int width = vcodec::group_width(a.version, control, (block[p0 + g / 4] >> ((g % 4) * 2)) & 3u);
+			const uint8_t* bytes = block + group[q * 16 + g];
+			if (width == 0 || width == 8)
+				for (uint32_t i = 0; i < 16; ++i)
+					out[i] = width ? bytes[i] : 0;
+			else
+				vcodec::unpack_group(bytes, width, out);
+		}
+	}
+	__syncwarp();
+
+	// deltas per column, the previous vertex taken as 0: lane l owns vertices 8 l .. 8 l + 7 (the staged bytes are dead now)
+	uint32_t* decoded = stage;
+	for (uint32_t k = 0; k < C; ++k)
+	{
+		const uint32_t channel = column_value(a.channel, k);
+		uint2 pl[4];
+		for (uint32_t j = 0; j < 4; ++j)
+			pl[j] = *reinterpret_cast<const uint2*>(planes + (4 * k + j) * kVertexBlock + lane * 8);
+		uint32_t v[8], acc = 0;
+		for (uint32_t t = 0; t < 8; ++t)
+		{
+			const uint32_t sh = (t & 3u) * 8u;
+			uint32_t bytes4 = 0;
+			for (uint32_t j = 0; j < 4; ++j)
+				bytes4 |= (((t < 4 ? pl[j].x : pl[j].y) >> sh) & 255u) << (8 * j);
+			acc = vcodec::combine(acc, vcodec::delta_term(bytes4, channel), channel);
+			v[t] = acc;
+		}
+		uint32_t x = acc;
+		for (uint32_t d = 1; d < 32; d <<= 1)
+		{
+			uint32_t y = __shfl_up_sync(full, x, d);
+			if (lane >= d)
+				x = vcodec::combine(y, x, channel);
+		}
+		uint32_t before = __shfl_up_sync(full, x, 1);
+		if (lane == 0)
+			before = 0;
+		for (uint32_t t = 0; t < 8; ++t)
+		{
+			const uint32_t i = lane * 8 + t;
+			const uint32_t value = vcodec::combine(before, v[t], channel);
+			decoded[padded_word(i, k, C)] = value;
+			if (i == n - 1)
+				a.carry[size_t(b) * C + k] = value;
+		}
+	}
+	__syncwarp();
+	uint32_t* dst = a.out + size_t(first) * C;
+	for (uint32_t w = lane; w < n * C; w += 32)
+		dst[w] = decoded[w + (w / C) / 8u];
+}
+
+// carry[b][k] = baseline[k] combined with the totals of blocks 0 .. b-1 (in place)
+template <uint32_t C>
+__global__ void __launch_bounds__(kCarryThreads) decode_vertex_carry_kernel(const VertexDecodeArgs a)
+{
+	const uint32_t full = 0xffffffffu;
+	__shared__ uint32_t s_warp[kCarryThreads / 32];
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	const uint32_t k = blockIdx.x, channel = column_value(a.channel, k);
+	uint32_t running = column_value(a.baseline, k);
+	for (uint32_t base = 0; base < a.blocks; base += kCarryThreads)
+	{
+		const uint32_t b = base + threadIdx.x;
+		uint32_t x = b < a.blocks ? a.carry[size_t(b) * C + k] : 0u;
+		for (uint32_t d = 1; d < 32; d <<= 1)
+		{
+			uint32_t y = __shfl_up_sync(full, x, d);
+			if (lane >= d)
+				x = vcodec::combine(y, x, channel);
+		}
+		if (lane == 31)
+			s_warp[warp] = x;
+		__syncthreads();
+		if (warp == 0)
+		{
+			uint32_t w = s_warp[lane];
+			for (uint32_t d = 1; d < 32; d <<= 1)
+			{
+				uint32_t y = __shfl_up_sync(full, w, d);
+				if (lane >= d)
+					w = vcodec::combine(y, w, channel);
+			}
+			s_warp[lane] = w;
+		}
+		__syncthreads();
+		uint32_t before = __shfl_up_sync(full, x, 1);
+		if (lane == 0)
+			before = warp ? s_warp[warp - 1] : 0u;
+		else if (warp)
+			before = vcodec::combine(s_warp[warp - 1], before, channel);
+		if (b < a.blocks)
+			a.carry[size_t(b) * C + k] = vcodec::combine(running, before, channel);
+		running = vcodec::combine(running, s_warp[kCarryThreads / 32 - 1], channel);
+		__syncthreads();
+	}
+}
+
+template <uint32_t C>
+__global__ void __launch_bounds__(kApplyThreads) decode_vertex_apply_kernel(const VertexDecodeArgs a)
+{
+	const size_t words = size_t(a.vertex_count) * C;
+	const size_t step = size_t(gridDim.x) * kApplyThreads; // a multiple of C: a thread keeps its column
+	const size_t w0 = size_t(blockIdx.x) * kApplyThreads + threadIdx.x;
+	const uint32_t k = uint32_t(w0 % C), channel = column_value(a.channel, k);
+	for (size_t w = w0; w < words; w += step)
+		a.out[w] = vcodec::combine(a.carry[w / C / kVertexBlock * C + k], a.out[w], channel);
+}
+
+// One meshlet codec block of `size` bytes -> vertexCount references (whole words, or two uint16 per word with shortRefs)
+// and then triangleCount * 3 index bytes from `out`; false when malformed.  Same reads, checks and order as the host's
+// decodeMeshletBlock.
+__device__ __forceinline__ bool decode_meshlet_block(const uint8_t* block, uint32_t size, uint32_t vertex_count, uint32_t triangle_count, bool short_refs, uint32_t* out)
+{
+	const uint32_t codes_size = (triangle_count + 1) / 2, ctrl_size = (vertex_count + 3) / 4;
+	const uint32_t gap_size = codes_size + ctrl_size < 16 ? 16 - (codes_size + ctrl_size) : 0;
+	if (size < codes_size + ctrl_size + gap_size)
+		return false;
+	const uint8_t* codes = block + size - codes_size;
+	const uint8_t* ctrl = codes - ctrl_size;
+	const uint32_t limit = size - codes_size - ctrl_size - gap_size; // deltas + extra occupy [0, limit)
+	uint32_t cursor = 0;
+
+	uint32_t previous = ~0u, pending = 0;
+	for (uint32_t group = 0; group * 4 < vertex_count; ++group)
+	{
+		const uint32_t control = ctrl[group];
+		for (uint32_t k = 0; k < 4; ++k)
+		{
+			const uint32_t width = control == 0xff ? 4 : (((control >> k) & 1u) | ((control >> (k + 3)) & 2u));
+			if (limit - cursor < width)
+				return false;
+			uint32_t value = 0;
+			for (uint32_t i = 0; i < width; ++i)
+				value |= uint32_t(block[cursor + i]) << (8 * i);
+			cursor += width;
+			previous = previous + ((value >> 1) ^ (0u - (value & 1u))) + 1;
+			const uint32_t i = group * 4 + k;
+			if (i < vertex_count)
+			{
+				if (!short_refs)
+					*out++ = previous;
+				else if (i & 1u)
+					*out++ = pending | (previous << 16);
+				else
+					pending = previous & 0xffffu;
+			}
+		}
+	}
+	if (short_refs && (vertex_count & 1u))
+		*out++ = pending;
+
+	uint32_t word = 0, filled = 0;
+	auto put = [&](uint32_t byte) {
+		word |= byte << (8 * filled);
+		if (++filled == 4)
+		{
+			*out++ = word;
+			word = 0;
+			filled = 0;
+		}
+	};
+	uint32_t h0 = 0, h1 = 0, h2 = 0; // the three previous triangles, a | b << 8 | c << 16, h0 the most recent
+	uint32_t unseen = 0;
+	for (uint32_t t = 0; t < triangle_count; ++t)
+	{
+		const uint32_t code = (codes[t / 2] >> ((t & 1) * 4)) & 15u;
+		uint32_t c[3];
+		if (code < 12)
+		{
+			const uint32_t from = code < 4 ? h0 : code < 8 ? h1 : h2;
+			c[0] = (code & 2) ? from >> 16 : from & 255u;
+			c[1] = (code & 2) ? (from >> 8) & 255u : from >> 16;
+			if (code & 1)
+			{
+				if (cursor >= limit)
+					return false;
+				c[2] = block[cursor++];
+			}
+			else
+				c[2] = unseen++ & 255u;
+		}
+		else
+			for (uint32_t j = 0; j < 3; ++j)
+			{
+				if (code > 12 + j)
+				{
+					if (cursor >= limit)
+						return false;
+					c[j] = block[cursor++];
+				}
+				else
+					c[j] = unseen++ & 255u;
+			}
+		put(c[0]);
+		put(c[1]);
+		put(c[2]);
+		h2 = h1;
+		h1 = h0;
+		h0 = c[0] | (c[1] << 8) | (c[2] << 16);
+	}
+	if (filled)
+		*out = word;
+	return cursor == limit;
+}
+
+__global__ void __launch_bounds__(kMeshletWarps * 32) decode_meshlets_kernel(const MeshletDecodeArgs a)
+{
+	__shared__ uint32_t s_stage[kMeshletWarps][kMeshletStageWords];
+	__shared__ uint32_t s_at[kMeshletWarps][32];
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	const uint32_t g = blockIdx.x * kMeshletWarps + warp, first = g * 32u;
+	if (first >= a.meshlet_count)
+		return; // whole warps
+	const uint32_t m = min(a.meshlet_count - first, 32u);
+	const uint32_t start = a.checkpoints[g], end = a.checkpoints[g + 1];
+	const uint32_t words = end / 4u + ((end & 3u) != 0) - start / 4u; // no wrap for offsets near 2^32
+	const uint8_t* span = a.stream + start;
+	if (words <= kMeshletStageWords)
+	{
+		const uint32_t* src = reinterpret_cast<const uint32_t*>(a.stream) + start / 4u;
+		for (uint32_t i = lane; i < words; i += 32)
+			s_stage[warp][i] = __ldg(src + i);
+		span = reinterpret_cast<const uint8_t*>(s_stage[warp]) + (start & 3u);
+	}
+	__syncwarp();
+	// the size chain of the group (the host walk checked that it adds up to the section's size)
+	if (lane == 0)
+		for (uint32_t i = 0, at = 0; i < m; ++i)
+		{
+			s_at[warp][i] = at;
+			at += 2u + (uint32_t(span[at]) | (uint32_t(span[at + 1]) << 8));
+		}
+	__syncwarp();
+	if (lane >= m)
+		return;
+	const uint32_t at = s_at[warp][lane];
+	const uint32_t size = uint32_t(span[at]) | (uint32_t(span[at + 1]) << 8);
+	const uint2 r = __ldg(reinterpret_cast<const uint2*>(a.records) + first + lane);
+	if (!decode_meshlet_block(span + at + 2, size, r.y & 255u, (r.y >> 8) & 255u, (r.y >> 16) & 1u, a.out + r.x))
+		atomicOr(a.corrupt, 1u);
+}
+
+} // namespace cache
+} // namespace nvc

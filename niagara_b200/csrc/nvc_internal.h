@@ -49,6 +49,9 @@ struct NvcContext
 	// nvc_cook_meshlets: job table and per-job scratch, grown as needed
 	void* cook_scratch = nullptr;
 	size_t cook_scratch_bytes = 0;
+	// nvc_scene_cache_read_device: the staged stream and its index, grown as needed
+	void* cache_scratch = nullptr;
+	size_t cache_scratch_bytes = 0;
 };
 
 namespace nvc
@@ -272,6 +275,30 @@ struct CookClrtArgs
 	uint32_t meshletvtx0_capacity;
 };
 cudaError_t launch_cook_meshlets_clrt(const CookClrtArgs& c, cudaStream_t stream);
+// nvc_scene_cache_read_device (nvc_cache_decode.cuh).  Every pointer is device memory; `stream` is the section as stored,
+// padded so that word loads that cover its last byte stay inside the allocation.
+struct VertexDecodeArgs
+{
+	const uint8_t* stream;
+	const uint32_t* block_start;  // [blocks + 1] (walk_vertex_stream)
+	const uint16_t* plane_offset; // [blocks][stride]
+	uint32_t* out;                // vertex_count * stride / 4 words
+	uint32_t* carry;              // [blocks][stride / 4]: block totals, then carries
+	uint32_t vertex_count, blocks, version;
+	uint32_t baseline[4]; // per 4-byte column: the baseline vertex of the stream's tail
+	uint32_t channel[4];  // per column: the channel byte of a v1 tail, 0 for v0
+};
+cudaError_t launch_decode_vertices(const VertexDecodeArgs& a, uint32_t stride, cudaStream_t stream);
+struct MeshletDecodeArgs
+{
+	const uint8_t* stream;
+	const uint32_t* checkpoints; // [groups of 32 meshlets + 1]: offset of the group's first size field (index_meshlet_stream)
+	const uint32_t* records;     // [meshlets][2]: dataOffset, vertexCount | triangleCount << 8 | shortRefs << 16
+	uint32_t* out;               // meshletdata words, zeroed
+	uint32_t meshlet_count;
+	uint32_t* corrupt; // set to 1 by a malformed block
+};
+cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);
 cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream);

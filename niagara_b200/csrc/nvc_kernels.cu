@@ -13,6 +13,7 @@
 #include "nvc_meshlets.cuh"
 #include "nvc_tma.cuh"
 #include "nvc_filter.cuh"
+#include "nvc_cache_decode.cuh"
 
 #include <cuda_runtime.h>
 #include <string.h>
@@ -3664,6 +3665,33 @@ cudaError_t clustercull_filter_occupancy(int* blocks_per_sm_early, int* blocks_p
 	if (e == cudaSuccess)
 		e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm_late, clustercull_filter_kernel<true, true, true, false, 1>, kClusterBlock, 0);
 	return e;
+}
+
+// nvc_scene_cache_read_device: the vertex codec's three passes (nvc_cache_decode.cuh)
+cudaError_t launch_decode_vertices(const VertexDecodeArgs& a, uint32_t stride, cudaStream_t stream)
+{
+	if (a.blocks == 0)
+		return cudaSuccess;
+	const size_t words = size_t(a.vertex_count) * (stride / 4);
+	const uint32_t apply_blocks = uint32_t(min(size_t(4096), (words + cache::kApplyThreads - 1) / cache::kApplyThreads));
+	const uint32_t grid = (a.blocks + cache::kVertexWarps - 1) / cache::kVertexWarps;
+	void (*blocks)(VertexDecodeArgs) = stride == 16 ? cache::decode_vertex_blocks_kernel<16> : cache::decode_vertex_blocks_kernel<8>;
+	void (*carry)(VertexDecodeArgs) = stride == 16 ? cache::decode_vertex_carry_kernel<4> : cache::decode_vertex_carry_kernel<2>;
+	void (*apply)(VertexDecodeArgs) = stride == 16 ? cache::decode_vertex_apply_kernel<4> : cache::decode_vertex_apply_kernel<2>;
+	blocks<<<grid, cache::kVertexWarps * 32, 0, stream>>>(a);
+	carry<<<stride / 4, cache::kCarryThreads, 0, stream>>>(a);
+	apply<<<apply_blocks, cache::kApplyThreads, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stream)
+{
+	if (a.meshlet_count == 0)
+		return cudaSuccess;
+	const uint32_t groups = (a.meshlet_count + 31) / 32;
+	void (*kernel)(MeshletDecodeArgs) = cache::decode_meshlets_kernel;
+	kernel<<<(groups + cache::kMeshletWarps - 1) / cache::kMeshletWarps, cache::kMeshletWarps * 32, 0, stream>>>(a);
+	return cudaGetLastError();
 }
 
 } // namespace nvc

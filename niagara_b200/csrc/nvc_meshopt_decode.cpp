@@ -22,6 +22,7 @@
 //   0xf0..0xfd  : restart, (b, c) slots from aux[code & 15]; a = next new vertex
 //   0xfe / 0xff : restart with an explicit aux byte (0xff: a explicit too); aux == 0 resets the vertex counter
 #include "../../include/niagara_cull.h"
+#include "nvc_meshopt_format.h"
 
 #include <string.h>
 
@@ -45,92 +46,68 @@ struct ByteReader
 	}
 };
 
-// 16 values of one byte plane
-bool read_byte_group(ByteReader& r, int width, uint8_t* out)
+// One byte plane of `count` values from r: control 3 = literals, 2 = zeros, else the selector header and its groups.
+// `group(g, width, bytes)` is called for every group of 16 values with the group_bytes(bytes, width) bytes it occupies;
+// false when the plane runs past r.end.  The decoder unpacks in `group`, the walk only measures.
+template <typename Group>
+bool walk_plane(ByteReader& r, int control, int version, uint32_t count, Group&& group)
 {
-	const uint8_t* packed;
-	if (width == 0)
-	{
-		memset(out, 0, 16);
+	const uint8_t* bytes;
+	if (control == 3)
+		return r.take(count, bytes);
+	if (control == 2)
 		return true;
-	}
-	if (width == 8)
-	{
-		if (!r.take(16, packed))
-			return false;
-		memcpy(out, packed, 16);
-		return true;
-	}
-	if (!r.take(size_t(2 * width), packed))
+	const uint32_t groups = (count + 15u) / 16u;
+	const uint8_t* selectors;
+	if (!r.take(vcodec::selector_bytes(groups), selectors))
 		return false;
-	// unpack without escapes first; a value equal to the all-ones code is then replaced by the next escape byte, in order
-	const uint8_t escape = uint8_t((1u << width) - 1u);
-	if (width == 4)
-		for (int i = 0; i < 8; ++i)
-		{
-			out[2 * i] = packed[i] >> 4;
-			out[2 * i + 1] = packed[i] & 15u;
-		}
-	else if (width == 2)
-		for (int i = 0; i < 4; ++i)
-		{
-			uint8_t b = packed[i];
-			out[4 * i] = b >> 6;
-			out[4 * i + 1] = (b >> 4) & 3u;
-			out[4 * i + 2] = (b >> 2) & 3u;
-			out[4 * i + 3] = b & 3u;
-		}
-	else // width 1: least significant bit first
-		for (int i = 0; i < 16; ++i)
-			out[i] = (packed[i >> 3] >> (i & 7)) & 1u;
-	for (int i = 0; i < 16; ++i)
-		if (out[i] == escape)
-		{
-			const uint8_t* e;
-			if (!r.take(1, e))
-				return false;
-			out[i] = *e;
-		}
+	for (uint32_t g = 0; g < groups; ++g)
+	{
+		const int width = vcodec::group_width(version, control, (selectors[g / 4] >> ((g % 4) * 2)) & 3u);
+		const size_t packed = width == 8 ? 16 : size_t(2 * width); // readable before the escapes can be counted
+		if (size_t(r.end - r.at) < packed || !r.take(vcodec::group_bytes(r.at, width), bytes))
+			return false;
+		group(g, width, bytes);
+	}
 	return true;
 }
 
 bool read_plane(ByteReader& r, int control, int version, uint32_t count, uint8_t* out /* room for count rounded up to 16 */)
 {
-	if (control == 3)
+	if (control == 3 || control == 2)
 	{
-		const uint8_t* lit;
-		if (!r.take(count, lit))
+		const uint8_t* lit = r.at;
+		if (!walk_plane(r, control, version, count, [](uint32_t, int, const uint8_t*) {}))
 			return false;
-		memcpy(out, lit, count);
+		if (control == 3)
+			memcpy(out, lit, count);
+		else
+			memset(out, 0, count);
 		return true;
 	}
-	if (control == 2)
-	{
-		memset(out, 0, count);
-		return true;
-	}
-	static const int kWidthsV0[4] = { 0, 2, 4, 8 };
-	static const int kWidthsV1[5] = { 0, 1, 2, 4, 8 };
-	const int* widths = version == 0 ? kWidthsV0 : kWidthsV1 + control;
-	uint32_t groups = (count + 15u) / 16u;
-	const uint8_t* selectors;
-	if (!r.take((groups + 3u) / 4u, selectors))
-		return false;
-	for (uint32_t g = 0; g < groups; ++g)
-	{
-		int sel = (selectors[g / 4] >> ((g % 4) * 2)) & 3;
-		if (!read_byte_group(r, widths[sel], out + g * 16))
-			return false;
-	}
-	return true;
+	return walk_plane(r, control, version, count, [&](uint32_t g, int width, const uint8_t* bytes) {
+		if (width == 0)
+			memset(out + g * 16, 0, 16);
+		else if (width == 8)
+			memcpy(out + g * 16, bytes, 16);
+		else
+			vcodec::unpack_group(bytes, width, out + g * 16);
+	});
 }
 
 inline uint32_t rotl(uint32_t v, int r) { return (v << r) | (v >> ((32 - r) & 31)); }
 
-} // namespace
+// The parts of a vertex stream around its blocks: the version, the baseline vertex and (v1) the channel bytes in the
+// tail, and the byte range the blocks must fill exactly.
+struct VertexStream
+{
+	int version;
+	const uint8_t* baseline;
+	const uint8_t* channels; // nullptr for v0 (channel 0 everywhere)
+	ByteReader blocks;
+};
 
-// 0 ok, negative NvcStatus otherwise
-int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint8_t* out)
+int open_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t stride, VertexStream& out)
 {
 	if (stride == 0 || stride > 256 || stride % 4 != 0)
 		return NVC_ERROR_INVALID_ARGUMENT;
@@ -144,15 +121,28 @@ int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t ver
 	const size_t tail_padded = tail < tail_min ? tail_min : tail;
 	if (stream_size - 1 < tail_padded)
 		return NVC_ERROR_CORRUPT;
+	out.version = version;
+	out.baseline = stream + stream_size - tail;
+	out.channels = version == 0 ? nullptr : stream + stream_size - tail + stride;
+	out.blocks = { stream + 1, stream + stream_size - tail_padded };
+	return NVC_OK;
+}
 
+} // namespace
+
+// 0 ok, negative NvcStatus otherwise
+int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint8_t* out)
+{
+	VertexStream vs;
+	int status = open_vertex_stream(stream, stream_size, stride, vs);
+	if (status != NVC_OK)
+		return status;
+	const int version = vs.version;
+	const uint8_t* channels = vs.channels;
 	uint8_t previous[256];
-	memcpy(previous, stream + stream_size - tail, stride);
-	const uint8_t* channels = version == 0 ? nullptr : stream + stream_size - tail + stride;
-
-	ByteReader r = { stream + 1, stream + stream_size - tail_padded };
-	uint32_t per_block = uint32_t((8192u / stride) & ~15u);
-	if (per_block > 256)
-		per_block = 256;
+	memcpy(previous, vs.baseline, stride);
+	ByteReader& r = vs.blocks;
+	const uint32_t per_block = vcodec::block_vertices(stride);
 
 	uint8_t planes[4][256 + 16];
 	for (uint32_t first = 0; first < vertex_count; first += per_block)
@@ -218,6 +208,54 @@ int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t ver
 		}
 		memcpy(previous, block + size_t(count - 1) * stride, stride);
 	}
+	return r.at == r.end ? NVC_OK : NVC_ERROR_CORRUPT;
+}
+
+// Indexes a vertex stream for the device decoder (nvc_cache_decode.cuh) without decoding it: for every block the offset
+// of its first byte from the start of the stream (block_start[blocks] = where the blocks end) and, for each of its
+// `stride` byte planes in stream order, the plane's offset from the block's start.  Only sizes are read: control bytes,
+// selector headers, and the escape counts of the packed groups.  Walks the structure decode_vertex_stream decodes and
+// returns the status it returns on every stream, so a stream the walk accepts decodes without a check on the device.
+// Strides up to 16 (a block then spans less than 2^16 bytes); streams under 4 GiB, NVC_ERROR_UNSUPPORTED otherwise.
+int walk_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint32_t* block_start, uint16_t* plane_offset,
+    VertexStreamTail* tail)
+{
+	if (stride > 16)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (stream_size > 0xffffffffull)
+		return NVC_ERROR_UNSUPPORTED; // block starts are 32-bit offsets
+	VertexStream vs;
+	int status = open_vertex_stream(stream, stream_size, stride, vs);
+	if (status != NVC_OK)
+		return status;
+	tail->version = vs.version;
+	tail->baseline = vs.baseline;
+	tail->channels = vs.channels;
+	ByteReader& r = vs.blocks;
+	const uint32_t per_block = vcodec::block_vertices(stride);
+	auto nothing = [](uint32_t, int, const uint8_t*) {};
+	uint32_t b = 0;
+	for (uint32_t first = 0; first < vertex_count; first += per_block, ++b)
+	{
+		uint32_t count = vertex_count - first < per_block ? vertex_count - first : per_block;
+		const uint8_t* block = r.at;
+		block_start[b] = uint32_t(block - stream);
+		const uint8_t* control = nullptr;
+		if (vs.version != 0 && !r.take(stride / 4, control))
+			return NVC_ERROR_CORRUPT;
+		for (uint32_t q = 0; q < stride; ++q)
+		{
+			plane_offset[size_t(b) * stride + q] = uint16_t(r.at - block);
+			uint32_t ctrl = control ? (control[q / 4] >> ((q % 4) * 2)) & 3u : 0u;
+			if (!walk_plane(r, int(ctrl), vs.version, count, nothing))
+				return NVC_ERROR_CORRUPT;
+		}
+		// decode_vertex_stream rejects a channel it has no delta for at the first block
+		for (uint32_t k = 0; vs.channels && b == 0 && k < stride / 4; ++k)
+			if ((vs.channels[k] & 3) == 3)
+				return NVC_ERROR_CORRUPT;
+	}
+	block_start[b] = uint32_t(r.at - stream);
 	return r.at == r.end ? NVC_OK : NVC_ERROR_CORRUPT;
 }
 

@@ -19,15 +19,9 @@
 //   vertex; nibble >= 12 starts a new triangle with nibble - 12 explicit bytes for its (a, b, c) — explicit bytes
 //   come first, then consecutive unseen vertices.
 #include "../../include/niagara_cull.h"
+#include "nvc_meshopt_format.h"
 
 #include <string.h>
-
-namespace nvc
-{
-// nvc_meshopt_decode.cpp
-int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint8_t* out);
-int decode_index_stream(const uint8_t* stream, size_t stream_size, uint32_t index_count, uint32_t* out);
-} // namespace nvc
 
 namespace
 {
@@ -240,6 +234,49 @@ extern "C" NVC_API int nvc_scene_cache_read(const void* file, size_t file_size, 
 	}
 	return NVC_OK;
 }
+
+namespace nvc
+{
+
+int index_meshlet_stream(const void* file, size_t file_size, const NvcSceneCacheInfo* info, uint32_t* checkpoints, uint32_t* records)
+{
+	const NvcSceneCacheSection& md = info->sections[NVC_CACHE_MESHLETDATA];
+	const NvcSceneCacheSection& ms = info->sections[NVC_CACHE_MESHLETS];
+	const uint32_t count = info->header.meshletCount;
+	if (ms.offset > file_size || uint64_t(count) * sizeof(NvcMeshlet) > file_size - ms.offset || md.offset > file_size || md.stored_bytes > file_size - md.offset)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (md.stored_bytes > 0xffffffffull)
+		return NVC_ERROR_UNSUPPORTED; // checkpoints are 32-bit offsets
+	const uint8_t* base = static_cast<const uint8_t*>(file);
+	const uint8_t* p = base + md.offset;
+	uint64_t at = 0, end = 0;
+	bool ordered = true;
+	for (uint32_t i = 0; i < count; ++i)
+	{
+		NvcMeshlet m;
+		memcpy(&m, base + ms.offset + size_t(i) * sizeof(NvcMeshlet), sizeof(m));
+		uint64_t ref_words = m.shortRefs ? (uint64_t(m.vertexCount) + 1) / 2 : m.vertexCount;
+		uint64_t words = ref_words + (uint64_t(m.triangleCount) * 3 + 3) / 4;
+		// nvc_scene_cache_parse checks both of these: an info they fail does not describe this file
+		if (uint64_t(m.dataOffset) + words > md.count || at + 2 > md.stored_bytes)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		ordered = ordered && m.dataOffset >= end;
+		end = m.dataOffset + words;
+		if (i % kMeshletGroup == 0)
+			checkpoints[i / kMeshletGroup] = uint32_t(at);
+		records[2 * size_t(i)] = m.dataOffset;
+		records[2 * size_t(i) + 1] = uint32_t(m.vertexCount) | (uint32_t(m.triangleCount) << 8) | (m.shortRefs ? 1u << 16 : 0u);
+		uint16_t n;
+		memcpy(&n, p + at, 2);
+		at += 2 + uint64_t(n);
+	}
+	if (at != md.stored_bytes)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	checkpoints[(count + kMeshletGroup - 1) / kMeshletGroup] = uint32_t(at);
+	return ordered ? NVC_OK : NVC_ERROR_UNSUPPORTED;
+}
+
+} // namespace nvc
 
 extern "C" NVC_API int nvc_decode_vertex_stream(void* dst, uint32_t vertex_count, uint32_t vertex_size, const void* stream, size_t stream_size)
 {

@@ -1,0 +1,209 @@
+// nvc_scene_cache_device.cpp — nvc_scene_cache_read into device memory.  The vertex streams (VERTICES, MESHLETVTX0) and
+// the per-meshlet stream (MESHLETDATA) go up as stored, with an index the host finds by walking their sizes only
+// (walk_vertex_stream, index_meshlet_stream), and are decoded by the kernels of nvc_cache_decode.cuh.  Raw sections are
+// copied up; INDICES is decoded on the host (the index codec is one sequential FIFO state machine) and copied up.
+#include "nvc_internal.h"
+#include "nvc_meshopt_format.h"
+
+#include <string.h>
+
+#include <vector>
+
+namespace
+{
+
+int cuda_fail(NvcContext* ctx, cudaError_t e)
+{
+	ctx->last_error = std::string("nvc_scene_cache_read_device: ") + cudaGetErrorString(e);
+	return e == cudaErrorMemoryAllocation ? NVC_ERROR_OUT_OF_MEMORY : NVC_ERROR_CUDA;
+}
+
+// Sub-allocations of the context's cache scratch, each starting 256-byte aligned.  The staged stream is taken last, so a
+// scratch allocated for this call ends where the stream's last word does.
+struct Plan
+{
+	size_t bytes = 0;
+	size_t take(size_t n)
+	{
+		size_t at = (bytes + 255) & ~size_t(255);
+		bytes = at + n;
+		return at;
+	}
+};
+
+// grows the context's scratch to `bytes`; its previous user has finished (the call synchronised the device)
+cudaError_t reserve(NvcContext* ctx, size_t bytes)
+{
+	if (bytes <= ctx->cache_scratch_bytes)
+		return cudaSuccess;
+	cudaFree(ctx->cache_scratch);
+	ctx->cache_scratch = nullptr;
+	ctx->cache_scratch_bytes = 0;
+	cudaError_t e = cudaMalloc(&ctx->cache_scratch, bytes);
+	if (e == cudaSuccess)
+		ctx->cache_scratch_bytes = bytes;
+	return e;
+}
+
+// a stored stream staged in whole words: the kernels' word loads cover its last byte and go no further
+size_t staged_bytes(uint64_t stored)
+{
+	return size_t((stored + 3) & ~uint64_t(3));
+}
+
+// A copy from pageable host memory may return before its DMA has landed, and it is not ordered with a non-blocking
+// `stream`: callers synchronise the device after their uploads, before a kernel reads them or the call returns.
+cudaError_t upload(void* dst, const void* src, size_t n)
+{
+	return n ? cudaMemcpy(dst, src, n, cudaMemcpyHostToDevice) : cudaSuccess;
+}
+
+int read_vertices(NvcContext* ctx, cudaStream_t stream, const uint8_t* data, const NvcSceneCacheSection& sec, uint32_t vertex_count, uint32_t stride, void* dst)
+{
+	const uint32_t blocks = (vertex_count + nvc::vcodec::block_vertices(stride) - 1) / nvc::vcodec::block_vertices(stride);
+	std::vector<uint32_t> block_start(size_t(blocks) + 1);
+	std::vector<uint16_t> plane_offset(size_t(blocks) * stride);
+	nvc::VertexStreamTail tail;
+	int status = nvc::walk_vertex_stream(data, sec.stored_bytes, vertex_count, stride, block_start.data(), plane_offset.data(), &tail);
+	if (status != NVC_OK)
+		return status;
+
+	Plan plan;
+	const size_t o_start = plan.take(block_start.size() * 4), o_plane = plan.take(plane_offset.size() * 2);
+	const size_t o_carry = plan.take(size_t(blocks) * stride), o_stream = plan.take(staged_bytes(sec.stored_bytes));
+	cudaError_t e = reserve(ctx, plan.bytes);
+	char* base = static_cast<char*>(ctx->cache_scratch);
+	if (e == cudaSuccess)
+		e = upload(base + o_stream, data, sec.stored_bytes);
+	if (e == cudaSuccess)
+		e = upload(base + o_start, block_start.data(), block_start.size() * 4);
+	if (e == cudaSuccess)
+		e = upload(base + o_plane, plane_offset.data(), plane_offset.size() * 2);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e);
+
+	nvc::VertexDecodeArgs a;
+	memset(&a, 0, sizeof(a));
+	a.stream = reinterpret_cast<const uint8_t*>(base + o_stream);
+	a.block_start = reinterpret_cast<const uint32_t*>(base + o_start);
+	a.plane_offset = reinterpret_cast<const uint16_t*>(base + o_plane);
+	a.out = static_cast<uint32_t*>(dst);
+	a.carry = reinterpret_cast<uint32_t*>(base + o_carry);
+	a.vertex_count = vertex_count;
+	a.blocks = blocks;
+	a.version = uint32_t(tail.version);
+	memcpy(a.baseline, tail.baseline, stride);
+	for (uint32_t k = 0; k < stride / 4; ++k)
+		a.channel[k] = tail.channels ? tail.channels[k] : 0u;
+	e = nvc::launch_decode_vertices(a, stride, stream);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e);
+}
+
+int read_meshletdata(NvcContext* ctx, cudaStream_t stream, const void* file, size_t file_size, const NvcSceneCacheInfo* info, void* dst)
+{
+	const NvcSceneCacheSection& sec = info->sections[NVC_CACHE_MESHLETDATA];
+	const uint32_t count = info->header.meshletCount;
+	std::vector<uint32_t> checkpoints((count + nvc::kMeshletGroup - 1) / nvc::kMeshletGroup + 1);
+	std::vector<uint32_t> records(size_t(count) * 2);
+	int status = nvc::index_meshlet_stream(file, file_size, info, checkpoints.data(), records.data());
+	if (status != NVC_OK)
+		return status;
+
+	Plan plan;
+	const size_t o_check = plan.take(checkpoints.size() * 4), o_records = plan.take(records.size() * 4), o_flag = plan.take(4);
+	const size_t o_stream = plan.take(staged_bytes(sec.stored_bytes));
+	cudaError_t e = reserve(ctx, plan.bytes);
+	char* base = static_cast<char*>(ctx->cache_scratch);
+	if (e == cudaSuccess)
+		e = upload(base + o_stream, static_cast<const uint8_t*>(file) + sec.offset, sec.stored_bytes);
+	if (e == cudaSuccess)
+		e = upload(base + o_check, checkpoints.data(), checkpoints.size() * 4);
+	if (e == cudaSuccess)
+		e = upload(base + o_records, records.data(), records.size() * 4);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	// as the host read: bytes no meshlet writes (padding, the unused half of an odd shortRefs word) are 0
+	if (e == cudaSuccess && sec.decoded_bytes)
+		e = cudaMemsetAsync(dst, 0, sec.decoded_bytes, stream);
+	if (e == cudaSuccess)
+		e = cudaMemsetAsync(base + o_flag, 0, 4, stream);
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e);
+
+	nvc::MeshletDecodeArgs a;
+	a.stream = reinterpret_cast<const uint8_t*>(base + o_stream);
+	a.checkpoints = reinterpret_cast<const uint32_t*>(base + o_check);
+	a.records = reinterpret_cast<const uint32_t*>(base + o_records);
+	a.out = static_cast<uint32_t*>(dst);
+	a.meshlet_count = count;
+	a.corrupt = reinterpret_cast<uint32_t*>(base + o_flag);
+	e = nvc::launch_decode_meshlets(a, stream);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	uint32_t corrupt = 0;
+	if (e == cudaSuccess)
+		e = cudaMemcpy(&corrupt, a.corrupt, 4, cudaMemcpyDeviceToHost);
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e);
+	return corrupt ? NVC_ERROR_CORRUPT : NVC_OK;
+}
+
+} // namespace
+
+extern "C" NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream, const void* file, size_t file_size, const NvcSceneCacheInfo* info, int section, void* dst,
+    size_t dst_bytes)
+{
+	if (!ctx || !file || !info || section < 0 || section >= NVC_CACHE_SECTION_COUNT || (!dst && dst_bytes) || (reinterpret_cast<uintptr_t>(dst) & 3u))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	const NvcSceneCacheSection& sec = info->sections[section];
+	if (dst_bytes < sec.decoded_bytes || sec.offset > file_size || sec.stored_bytes > file_size - sec.offset)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	int current = -1;
+	if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
+	{
+		ctx->last_error = "the context's CUDA device is not the calling thread's current device";
+		return NVC_ERROR_INVALID_ARGUMENT;
+	}
+	const uint8_t* data = static_cast<const uint8_t*>(file) + sec.offset;
+	const cudaStream_t s = static_cast<cudaStream_t>(stream);
+	// the caller's earlier work on `stream` and the previous call's use of the scratch finish before the copies below,
+	// which are not ordered with `stream` (see upload)
+	cudaError_t e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e);
+
+	if (!sec.compressed)
+	{
+		if (sec.decoded_bytes > sec.stored_bytes)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		e = upload(dst, data, sec.decoded_bytes);
+		if (e == cudaSuccess)
+			e = cudaDeviceSynchronize();
+		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e);
+	}
+	// the kernels and their index address the staged stream with 32-bit offsets
+	if (section != NVC_CACHE_INDICES && sec.stored_bytes > 0xffffffffull)
+		return NVC_ERROR_UNSUPPORTED;
+	if (section == NVC_CACHE_VERTICES)
+		return read_vertices(ctx, s, data, sec, sec.count, 16, dst);
+	if (section == NVC_CACHE_MESHLETVTX0) // uint16 x 4 per element of the stream
+		return sec.count % 4 ? NVC_ERROR_CORRUPT : read_vertices(ctx, s, data, sec, sec.count / 4, 8, dst);
+	if (section == NVC_CACHE_INDICES)
+	{
+		std::vector<uint32_t> indices(sec.count);
+		int status = nvc::decode_index_stream(data, sec.stored_bytes, sec.count, indices.data());
+		if (status != NVC_OK)
+			return status;
+		e = upload(dst, indices.data(), sec.decoded_bytes);
+		if (e == cudaSuccess)
+			e = cudaDeviceSynchronize();
+		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e);
+	}
+	if (section != NVC_CACHE_MESHLETDATA)
+		return NVC_ERROR_UNSUPPORTED;
+	return read_meshletdata(ctx, s, file, file_size, info, dst);
+}

@@ -73,6 +73,7 @@ SIGNATURES = [
     ("nvc_host_pass_data", None, [ctypes.POINTER(CullData), ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(CullData)]),
     ("nvc_scene_cache_parse", ctypes.c_int, [c_void_p, ctypes.c_size_t, ctypes.POINTER(SceneCacheInfo)]),
     ("nvc_scene_cache_read", ctypes.c_int, [c_void_p, ctypes.c_size_t, ctypes.POINTER(SceneCacheInfo), ctypes.c_int, c_void_p, ctypes.c_size_t]),
+    ("nvc_scene_cache_read_device", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_size_t, ctypes.POINTER(SceneCacheInfo), ctypes.c_int, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_vertex_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_index_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_meshlet_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),

@@ -1,12 +1,13 @@
 """Reader of the reference's scene cache (.cache v7, src/scenecache.cpp) through the C ABI (nvc_scene_cache_*):
-SURVEY §8(f) row N2 — the on-disk format that feeds the visibility path.  Host only."""
+SURVEY §8(f) row N2 — the on-disk format that feeds the visibility path.  `section` decodes on the host;
+`section_device` reads a section straight into device memory, decoding the vertex and meshlet streams on the GPU."""
 import ctypes
 import mmap
 
 import numpy as np
 
 from . import host, layout
-from .lib import NvcError, load_library
+from .lib import NvcError, check, load_library
 
 _DTYPES = {
     "meshlets": layout.MESHLET_DTYPE,
@@ -37,6 +38,7 @@ class SceneCache:
         if status != 0:
             raise NvcError("%s: %s" % (path, self._lib.nvc_status_string(status).decode()))
         self.header = self.info.header
+        self._contexts = {}  # device index -> NvcContext of section_device
 
     def _address(self):
         if self._buf is not None:
@@ -59,11 +61,39 @@ class SceneCache:
             return [bytes(raw[i * 256 : (i + 1) * 256]).split(b"\0", 1)[0].decode() for i in range(sec.count)]
         return raw.view(_DTYPES[name]) if name in _DTYPES else raw
 
+    def section_device(self, name, device="cuda"):
+        """The section's decoded bytes as a torch.uint8 tensor on `device`, equal to `section(name)`'s bytes
+        (nvc_scene_cache_read_device: the compressed vertex streams and meshlet data go up as stored and are decoded by
+        kernels; indices are decoded on the host).  Runs on the device's current stream and synchronises the device."""
+        import torch
+
+        idx = layout.CACHE_SECTIONS.index(name)
+        sec = self.info.sections[idx]
+        dev = torch.device(device)
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        out = torch.empty(int(sec.decoded_bytes), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            ctx = self._contexts.get(dev.index)
+            if ctx is None:
+                ctx = ctypes.c_void_p()
+                check(self._lib.nvc_create(dev.index, None, ctypes.byref(ctx)), None, "nvc_create")
+                self._contexts[dev.index] = ctx
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            status = self._lib.nvc_scene_cache_read_device(ctx, stream, self._address(), self.size, ctypes.byref(self.info), idx, out.data_ptr() if out.numel() else None, out.numel())
+        if status != 0:
+            detail = self._lib.nvc_last_error(ctx).decode()
+            raise NvcError("%s[%s]: %s%s" % (self.path, name, self._lib.nvc_status_string(status).decode(), " (%s)" % detail if detail else ""))
+        return out
+
     def camera(self):
         c = self.header.camera
         return host.make_camera(tuple(c.position), tuple(c.orientation), float(c.fovY), float(c.znear))
 
     def close(self):
+        for ctx in self._contexts.values():
+            self._lib.nvc_destroy(ctx)
+        self._contexts = {}
         self._view = None
         self._map.close()
         self._file.close()
