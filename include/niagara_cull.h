@@ -470,6 +470,44 @@ typedef struct NvcSceneCacheInfo
 NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream, const void* file, size_t file_size, const NvcSceneCacheInfo* info, int section,
     void* dst, size_t dst_bytes);
 
+/* What nvc_scene_cache_write stores: the header fields the caller chooses, and per section (NvcSceneCacheSectionId) a pointer
+ * and an element count in the reader's units (NvcSceneCacheSection.count: MESHLETVTX0 in uint16 elements, OMM data and
+ * indices in bytes, texture paths in 256-byte records).  Bit s of device_sections says that data[s] is device memory of the
+ * context's device (4-byte aligned); any section may be, and each other pointer is host memory.  A section with count 0 may
+ * have a NULL pointer. */
+typedef struct NvcSceneCacheWriteDesc
+{
+	uint64_t hashMeta;
+	uint32_t clrtMode, compressed, ommStates;
+	uint32_t device_sections;
+	NvcCamera camera;
+	float sunDirection[3];
+	const void* data[NVC_CACHE_SECTION_COUNT];
+	uint32_t count[NVC_CACHE_SECTION_COUNT];
+} NvcSceneCacheWriteDesc;
+
+/* Host: a size of the file nvc_scene_cache_write makes from `desc` that always suffices (the codecs' worst cases). */
+NVC_API int nvc_scene_cache_write_bound(const NvcSceneCacheWriteDesc* desc, size_t* bytes);
+/* The file saveSceneCache (src/scenecache.cpp:119-203) writes for these arrays, byte for byte, into the HOST buffer file_out
+ * (capacity >= nvc_scene_cache_write_bound); *file_size = its length.  The caller writes the file.
+ *   header      zero padding, meshletMaxVertices 64 / meshletMaxTriangles 96, the compressed byte counts when compressed
+ *   compressed  VERTICES and MESHLETVTX0 by the vertex codec v1 at level 2 (strides 16 and 8; an empty stream is 25 bytes),
+ *               INDICES by the index codec v1, MESHLETDATA as one uint16 size and one meshlet codec block per Meshlet, the
+ *               block encoding its vertexCount references (widened from uint16 when shortRefs) and triangleCount * 3 bytes
+ *   other       copied; texture paths as strncpy(record, path, 255) into a zeroed record
+ * The vertex and meshlet streams are encoded by kernels on `stream` (inputs in host memory are copied up first), the index
+ * stream on the host while they run (indices in device memory are copied down first).  Uncompressed writes run no kernel,
+ * and ctx may be NULL when no section is in device memory and nothing is encoded on the device.  Refused before
+ * anything is written to file_out:
+ *   NVC_ERROR_INVALID_ARGUMENT  a capacity below the bound; a device pointer, or compressed vertex / meshlet data, without
+ *                               a context; a misaligned device pointer; compressed with an index count that is not a
+ *                               multiple of 3 or a MESHLETVTX0 count that is not a multiple of 4; a meshlet whose words lie
+ *                               outside meshletdata or whose counts pass 64 vertices / 96 triangles (found on the device)
+ *   NVC_ERROR_UNSUPPORTED       a compressed stream of 4 GiB or more (the header's byte counts are 32-bit)
+ * Scratch is context-owned and grows as needed; the call synchronises the device, so it belongs at load time, outside
+ * stream capture. */
+NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, const NvcSceneCacheWriteDesc* desc, void* file_out, size_t capacity, size_t* file_size);
+
 /* The three meshopt stream decoders on their own (the same streams appear in glTF EXT_meshopt_compression buffers):
  *   vertex codec v0 / v1   -> dst[vertex_count * vertex_size], vertex_size a multiple of 4, <= 256
  *   index codec v0 / v1    -> dst[index_count] uint32, index_count a multiple of 3 (triangles come back rotated)

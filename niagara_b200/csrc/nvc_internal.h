@@ -49,7 +49,7 @@ struct NvcContext
 	// nvc_cook_meshlets: job table and per-job scratch, grown as needed
 	void* cook_scratch = nullptr;
 	size_t cook_scratch_bytes = 0;
-	// nvc_scene_cache_read_device: the staged stream and its index, grown as needed
+	// nvc_scene_cache_read_device: the staged stream and its index; nvc_scene_cache_write: the inputs and encoded streams; grown as needed
 	void* cache_scratch = nullptr;
 	size_t cache_scratch_bytes = 0;
 };
@@ -299,6 +299,55 @@ struct MeshletDecodeArgs
 	uint32_t* corrupt; // set to 1 by a malformed block
 };
 cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stream);
+// Sub-allocations of the context's cache scratch (nvc_scene_cache_read_device, nvc_scene_cache_write), each 256-byte aligned
+struct ScratchPlan
+{
+	size_t bytes = 0;
+	size_t take(size_t n)
+	{
+		size_t at = (bytes + 255) & ~size_t(255);
+		bytes = at + n;
+		return at;
+	}
+};
+// grows the context's cache scratch to `bytes`; its previous user has finished (the caller synchronised the device)
+inline cudaError_t reserve_cache_scratch(NvcContext* ctx, size_t bytes)
+{
+	if (bytes <= ctx->cache_scratch_bytes)
+		return cudaSuccess;
+	cudaFree(ctx->cache_scratch);
+	ctx->cache_scratch = nullptr;
+	ctx->cache_scratch_bytes = 0;
+	cudaError_t e = cudaMalloc(&ctx->cache_scratch, bytes);
+	if (e == cudaSuccess)
+		ctx->cache_scratch_bytes = bytes;
+	return e;
+}
+// nvc_scene_cache_write (nvc_cache_encode.cuh).  Every pointer is device memory.
+constexpr uint32_t kVertexBlockEncode = 256; // vcodec::block_vertices of strides 8 and 16
+struct VertexEncodeArgs
+{
+	const uint8_t* vertices;       // vertex_count * stride bytes, 4-byte aligned
+	uint32_t vertex_count, blocks; // blocks of kVertexBlockEncode vertices
+	unsigned long long* estimate;  // [stride / 4][2]: per column the channel estimate's byte counts of channels 0 and 1
+	uint32_t* block_bytes;         // [blocks]: each block's size (measure pass)
+	unsigned long long* offsets;   // [blocks + 1]: their exclusive scan, then the total
+	uint8_t* out;                  // the stream: header byte, blocks, tail
+};
+// estimate, measure, scan, write; the stream takes 1 + offsets[blocks] + 24 bytes.  vertex_count > 0.
+cudaError_t launch_encode_vertices(const VertexEncodeArgs& a, uint32_t stride, cudaStream_t stream);
+struct MeshletEncodeArgs
+{
+	const NvcMeshlet* meshlets;
+	const uint32_t* meshletdata;
+	uint32_t meshlet_count, meshletdata_count;
+	uint32_t* block_bytes;       // [meshlets]: 2 + each meshlet's block size (measure pass)
+	unsigned long long* offsets; // [meshlets + 1]: their exclusive scan, then the section's size
+	uint8_t* out;                // the MESHLETDATA section
+	uint32_t* invalid;           // zeroed; set to 1 by a meshlet outside meshletdata or past 64 vertices / 96 triangles
+};
+// measure, scan, write (the write pass skips the meshlets the measure pass flagged)
+cudaError_t launch_encode_meshlets(const MeshletEncodeArgs& a, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);
 cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream);

@@ -14,6 +14,7 @@
 #include "nvc_tma.cuh"
 #include "nvc_filter.cuh"
 #include "nvc_cache_decode.cuh"
+#include "nvc_cache_encode.cuh"
 
 #include <cuda_runtime.h>
 #include <string.h>
@@ -3691,6 +3692,44 @@ cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stre
 	const uint32_t groups = (a.meshlet_count + 31) / 32;
 	void (*kernel)(MeshletDecodeArgs) = cache::decode_meshlets_kernel;
 	kernel<<<(groups + cache::kMeshletWarps - 1) / cache::kMeshletWarps, cache::kMeshletWarps * 32, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
+// nvc_scene_cache_write: the vertex codec's estimate, measure, scan and write passes (nvc_cache_encode.cuh)
+cudaError_t launch_encode_vertices(const VertexEncodeArgs& a, uint32_t stride, cudaStream_t stream)
+{
+	cudaError_t e = cudaMemsetAsync(a.estimate, 0, sizeof(unsigned long long) * 2 * (stride / 4), stream);
+	if (e != cudaSuccess)
+		return e;
+	const uint32_t grid = (a.blocks + cache::kEncodeWarps - 1) / cache::kEncodeWarps;
+	const size_t items = (size_t(a.vertex_count) + 3 * kVertexBlockEncode - 1) / (3 * kVertexBlockEncode) * 16 * (stride / 4);
+	const uint32_t estimate_blocks = uint32_t(min(size_t(4096), (items + cache::kEstimateThreads - 1) / cache::kEstimateThreads));
+	void (*estimate)(VertexEncodeArgs) = stride == 16 ? cache::encode_vertex_estimate_kernel<16> : cache::encode_vertex_estimate_kernel<8>;
+	void (*measure)(VertexEncodeArgs) = stride == 16 ? cache::encode_vertex_blocks_kernel<16, false> : cache::encode_vertex_blocks_kernel<8, false>;
+	void (*write)(VertexEncodeArgs) = stride == 16 ? cache::encode_vertex_blocks_kernel<16, true> : cache::encode_vertex_blocks_kernel<8, true>;
+	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	if (a.vertex_count > 1) // one vertex keeps channel 0 everywhere
+		estimate<<<estimate_blocks, cache::kEstimateThreads, 0, stream>>>(a);
+	measure<<<grid, cache::kEncodeWarps * 32, 0, stream>>>(a);
+	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_bytes, a.blocks, a.offsets);
+	write<<<grid, cache::kEncodeWarps * 32, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_encode_meshlets(const MeshletEncodeArgs& a, cudaStream_t stream)
+{
+	cudaError_t e = cudaMemsetAsync(a.invalid, 0, 4, stream);
+	if (e != cudaSuccess)
+		return e;
+	const uint32_t grid = (a.meshlet_count + cache::kMeshletEncodeThreads - 1) / cache::kMeshletEncodeThreads;
+	void (*measure)(MeshletEncodeArgs) = cache::encode_meshlets_kernel<false>;
+	void (*write)(MeshletEncodeArgs) = cache::encode_meshlets_kernel<true>;
+	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	if (a.meshlet_count)
+		measure<<<grid, cache::kMeshletEncodeThreads, 0, stream>>>(a);
+	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_bytes, a.meshlet_count, a.offsets);
+	if (a.meshlet_count)
+		write<<<grid, cache::kMeshletEncodeThreads, 0, stream>>>(a);
 	return cudaGetLastError();
 }
 

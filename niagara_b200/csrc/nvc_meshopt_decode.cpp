@@ -262,20 +262,6 @@ int walk_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t verte
 namespace
 {
 
-struct Ring16
-{
-	uint32_t slot[16];
-	uint32_t head = 0;
-	Ring16() { memset(slot, 0xff, sizeof(slot)); }
-	// the slot is written even when the head does not advance — the encoder does the same, and both must agree
-	void put(uint32_t v, bool advance = true)
-	{
-		slot[head] = v;
-		head = (head + (advance ? 1u : 0u)) & 15u;
-	}
-	uint32_t back(uint32_t n) const { return slot[(head - n) & 15u]; } // back(1) = most recent
-};
-
 bool read_varint_delta(ByteReader& r, uint32_t& last)
 {
 	uint32_t value = 0;
@@ -312,7 +298,7 @@ int decode_index_stream(const uint8_t* stream, size_t stream_size, uint32_t inde
 	const uint8_t* aux = stream + stream_size - 16;
 	ByteReader r = { codes + triangles, aux };
 
-	Ring16 verts, edge_a, edge_b;
+	icodec::Ring16 verts, edge_a, edge_b;
 	auto push_edge = [&](uint32_t a, uint32_t b) {
 		edge_a.put(a);
 		edge_b.put(b);

@@ -6,6 +6,7 @@
 
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/niagara_cull.h"
 
@@ -127,6 +128,28 @@ NVC_CODEC_FN inline uint32_t combine(uint32_t a, uint32_t b, uint32_t channel)
 
 } // namespace vcodec
 
+namespace icodec
+{
+
+// One of the index codec's 16-entry FIFOs (vertices; edges as two rings pushed together), as the decoder keeps it.  The
+// encoder keeps the same rings, so that every slot it codes is the one the decoder will read.
+struct Ring16
+{
+	uint32_t slot[16];
+	uint32_t head = 0;
+	Ring16() { memset(slot, 0xff, sizeof(slot)); }
+	// the slot is written even when the head does not advance (a vertex re-read from the FIFO); the next put overwrites it
+	// before any lookup can reach it
+	void put(uint32_t v, bool advance = true)
+	{
+		slot[head] = v;
+		head = (head + (advance ? 1u : 0u)) & 15u;
+	}
+	uint32_t back(uint32_t n) const { return slot[(head - n) & 15u]; } // back(1) = most recent
+};
+
+} // namespace icodec
+
 // Where a vertex stream keeps its version, baseline vertex and (v1) channel bytes (channels nullptr for v0)
 struct VertexStreamTail
 {
@@ -141,6 +164,10 @@ int decode_index_stream(const uint8_t* stream, size_t stream_size, uint32_t inde
 int walk_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint32_t* block_start, uint16_t* plane_offset,
     VertexStreamTail* tail);
 
+// nvc_meshopt_encode.cpp (host): index codec v1 of index_count indices (a multiple of 3) into out[index_stream_bound]
+size_t index_stream_bound(size_t index_count);
+size_t encode_index_stream(const uint32_t* indices, size_t index_count, uint8_t* out);
+
 // nvc_scene_cache.cpp (host): the per-meshlet stream of a compressed MESHLETDATA section indexed for the device decoder,
 // without decoding it.  checkpoints[(meshletCount + kMeshletGroup - 1) / kMeshletGroup + 1]: the offset of every
 // kMeshletGroup-th meshlet's size field, then the section's size.  records[meshletCount][2]: dataOffset and
@@ -149,6 +176,9 @@ int walk_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t verte
 // owns whole words of the output, or when the section is 4 GiB or larger; NVC_ERROR_INVALID_ARGUMENT when `info` does not
 // describe the file.
 constexpr uint32_t kMeshletGroup = 32;
+
+// bytes per element of each section (NvcSceneCacheSectionId order), as the header counts them
+constexpr uint32_t kCacheElementSize[NVC_CACHE_SECTION_COUNT] = { 16, 4, 24, 4, 2, 208, 64, 48, 32, 24, 32, 1, 1, 4, 256 };
 int index_meshlet_stream(const void* file, size_t file_size, const NvcSceneCacheInfo* info, uint32_t* checkpoints, uint32_t* records);
 
 } // namespace nvc

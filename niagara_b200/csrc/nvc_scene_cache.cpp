@@ -26,8 +26,6 @@
 namespace
 {
 
-const uint32_t kElementSize[NVC_CACHE_SECTION_COUNT] = { 16, 4, 24, 4, 2, 208, 64, 48, 32, 24, 32, 1, 1, 4, 256 };
-
 // one meshlet block -> refs (ref_size 2 or 4 bytes each) and triangles (3 bytes each); false when malformed
 bool decodeMeshletBlock(const uint8_t* block, size_t size, uint32_t vertex_count, uint32_t triangle_count, uint32_t ref_size, uint8_t* refs_out, uint8_t* triangles_out)
 {
@@ -135,7 +133,7 @@ extern "C" NVC_API int nvc_scene_cache_parse(const void* file, size_t file_size,
 	{
 		NvcSceneCacheSection& sec = out->sections[s];
 		sec.count = counts[s];
-		sec.element_size = kElementSize[s];
+		sec.element_size = nvc::kCacheElementSize[s];
 		sec.decoded_bytes = uint64_t(sec.count) * sec.element_size;
 		sec.stored_bytes = sec.decoded_bytes;
 		if (h.compressed)

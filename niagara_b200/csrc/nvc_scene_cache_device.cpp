@@ -18,33 +18,6 @@ int cuda_fail(NvcContext* ctx, cudaError_t e)
 	return e == cudaErrorMemoryAllocation ? NVC_ERROR_OUT_OF_MEMORY : NVC_ERROR_CUDA;
 }
 
-// Sub-allocations of the context's cache scratch, each starting 256-byte aligned.  The staged stream is taken last, so a
-// scratch allocated for this call ends where the stream's last word does.
-struct Plan
-{
-	size_t bytes = 0;
-	size_t take(size_t n)
-	{
-		size_t at = (bytes + 255) & ~size_t(255);
-		bytes = at + n;
-		return at;
-	}
-};
-
-// grows the context's scratch to `bytes`; its previous user has finished (the call synchronised the device)
-cudaError_t reserve(NvcContext* ctx, size_t bytes)
-{
-	if (bytes <= ctx->cache_scratch_bytes)
-		return cudaSuccess;
-	cudaFree(ctx->cache_scratch);
-	ctx->cache_scratch = nullptr;
-	ctx->cache_scratch_bytes = 0;
-	cudaError_t e = cudaMalloc(&ctx->cache_scratch, bytes);
-	if (e == cudaSuccess)
-		ctx->cache_scratch_bytes = bytes;
-	return e;
-}
-
 // a stored stream staged in whole words: the kernels' word loads cover its last byte and go no further
 size_t staged_bytes(uint64_t stored)
 {
@@ -68,10 +41,10 @@ int read_vertices(NvcContext* ctx, cudaStream_t stream, const uint8_t* data, con
 	if (status != NVC_OK)
 		return status;
 
-	Plan plan;
+	nvc::ScratchPlan plan; // the staged stream is taken last: a scratch allocated for this call ends where its last word does
 	const size_t o_start = plan.take(block_start.size() * 4), o_plane = plan.take(plane_offset.size() * 2);
 	const size_t o_carry = plan.take(size_t(blocks) * stride), o_stream = plan.take(staged_bytes(sec.stored_bytes));
-	cudaError_t e = reserve(ctx, plan.bytes);
+	cudaError_t e = nvc::reserve_cache_scratch(ctx, plan.bytes);
 	char* base = static_cast<char*>(ctx->cache_scratch);
 	if (e == cudaSuccess)
 		e = upload(base + o_stream, data, sec.stored_bytes);
@@ -113,10 +86,10 @@ int read_meshletdata(NvcContext* ctx, cudaStream_t stream, const void* file, siz
 	if (status != NVC_OK)
 		return status;
 
-	Plan plan;
+	nvc::ScratchPlan plan;
 	const size_t o_check = plan.take(checkpoints.size() * 4), o_records = plan.take(records.size() * 4), o_flag = plan.take(4);
 	const size_t o_stream = plan.take(staged_bytes(sec.stored_bytes));
-	cudaError_t e = reserve(ctx, plan.bytes);
+	cudaError_t e = nvc::reserve_cache_scratch(ctx, plan.bytes);
 	char* base = static_cast<char*>(ctx->cache_scratch);
 	if (e == cudaSuccess)
 		e = upload(base + o_stream, static_cast<const uint8_t*>(file) + sec.offset, sec.stored_bytes);

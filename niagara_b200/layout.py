@@ -267,7 +267,21 @@ class SceneCacheInfo(ctypes.Structure):
     _fields_ = [("header", SceneCacheHeader), ("sections", SceneCacheSection * len(CACHE_SECTIONS))]
 
 
-assert ctypes.sizeof(SceneCacheHeader) == 160 and ctypes.sizeof(SceneCacheSection) == 40
+class SceneCacheWriteDesc(ctypes.Structure):  # nvc_scene_cache_write
+    _fields_ = [
+        ("hashMeta", ctypes.c_uint64),
+        ("clrtMode", ctypes.c_uint32),
+        ("compressed", ctypes.c_uint32),
+        ("ommStates", ctypes.c_uint32),
+        ("device_sections", ctypes.c_uint32),
+        ("camera", Camera),
+        ("sunDirection", ctypes.c_float * 3),
+        ("data", ctypes.c_void_p * len(CACHE_SECTIONS)),
+        ("count", ctypes.c_uint32 * len(CACHE_SECTIONS)),
+    ]
+
+
+assert ctypes.sizeof(SceneCacheHeader) == 160 and ctypes.sizeof(SceneCacheSection) == 40 and ctypes.sizeof(SceneCacheWriteDesc) == 256
 
 
 def load_nvcg(path):

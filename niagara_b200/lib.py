@@ -6,7 +6,7 @@ import ctypes
 import os
 
 from . import _build
-from .layout import Camera, CullData, CullOptions, GltfInfo, HiZ, Limits, SceneCacheInfo
+from .layout import Camera, CullData, CullOptions, GltfInfo, HiZ, Limits, SceneCacheInfo, SceneCacheWriteDesc
 
 _LIB = None
 
@@ -74,6 +74,8 @@ SIGNATURES = [
     ("nvc_scene_cache_parse", ctypes.c_int, [c_void_p, ctypes.c_size_t, ctypes.POINTER(SceneCacheInfo)]),
     ("nvc_scene_cache_read", ctypes.c_int, [c_void_p, ctypes.c_size_t, ctypes.POINTER(SceneCacheInfo), ctypes.c_int, c_void_p, ctypes.c_size_t]),
     ("nvc_scene_cache_read_device", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_size_t, ctypes.POINTER(SceneCacheInfo), ctypes.c_int, c_void_p, ctypes.c_size_t]),
+    ("nvc_scene_cache_write_bound", ctypes.c_int, [ctypes.POINTER(SceneCacheWriteDesc), ctypes.POINTER(ctypes.c_size_t)]),
+    ("nvc_scene_cache_write", ctypes.c_int, [c_void_p, c_void_p, ctypes.POINTER(SceneCacheWriteDesc), c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]),
     ("nvc_decode_vertex_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_index_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_meshlet_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),

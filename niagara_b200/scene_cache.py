@@ -1,6 +1,7 @@
-"""Reader of the reference's scene cache (.cache v7, src/scenecache.cpp) through the C ABI (nvc_scene_cache_*):
+"""Reader and writer of the reference's scene cache (.cache v7, src/scenecache.cpp) through the C ABI (nvc_scene_cache_*):
 SURVEY §8(f) row N2 — the on-disk format that feeds the visibility path.  `section` decodes on the host;
-`section_device` reads a section straight into device memory, decoding the vertex and meshlet streams on the GPU."""
+`section_device` reads a section straight into device memory, decoding the vertex and meshlet streams on the GPU;
+`write_scene_cache` makes the file saveSceneCache writes, encoding the vertex and meshlet streams on the GPU."""
 import ctypes
 import mmap
 
@@ -97,6 +98,71 @@ class SceneCache:
         self._view = None
         self._map.close()
         self._file.close()
+
+
+_ELEMENT_SIZE = dict(zip(layout.CACHE_SECTIONS, (16, 4, 24, 4, 2, 208, 64, 48, 32, 24, 32, 1, 1, 4, 256)))
+_WRITE_CONTEXTS = {}  # device index -> NvcContext of write_scene_cache
+
+
+def _write_context(lib, index):
+    ctx = _WRITE_CONTEXTS.get(index)
+    if ctx is None:
+        ctx = ctypes.c_void_p()
+        check(lib.nvc_create(index, None, ctypes.byref(ctx)), None, "nvc_create")
+        _WRITE_CONTEXTS[index] = ctx
+    return ctx
+
+
+def write_scene_cache(sections, compressed=True, hash_meta=0, clrt_mode=False, omm_states=0, camera=None, sun_direction=(0.0, 0.0, 0.0), device=None):
+    """The bytes of the scene cache saveSceneCache writes for `sections` (nvc_scene_cache_write).  `sections` maps names of
+    layout.CACHE_SECTIONS to numpy arrays or torch tensors (CUDA tensors are read where they lie), whose bytes are the
+    section's elements; missing sections are empty; "texture_paths" may also be a list of str.  `camera` is a
+    layout.Camera.  A compressed cache encodes the vertex and meshlet streams on `device` (default: the device of the
+    CUDA tensors given, else the current one), on its current stream; the call synchronises that device."""
+    lib = load_library()
+    desc = layout.SceneCacheWriteDesc()
+    desc.hashMeta, desc.clrtMode, desc.compressed, desc.ommStates = int(hash_meta), int(bool(clrt_mode)), int(bool(compressed)), int(omm_states)
+    if camera is not None:
+        desc.camera = camera
+    desc.sunDirection[:] = [float(x) for x in sun_direction]
+    keep = []
+    cuda_index = None
+    for name, value in sections.items():
+        idx = layout.CACHE_SECTIONS.index(name)
+        if name == "texture_paths" and isinstance(value, (list, tuple)):
+            value = np.frombuffer(b"".join(p.encode()[:256].ljust(256, b"\0") for p in value), np.uint8)
+        if hasattr(value, "is_cuda") and value.is_cuda:
+            value = value.contiguous()
+            cuda_index = value.device.index if cuda_index is None else cuda_index
+            if value.device.index != cuda_index:
+                raise NvcError("write_scene_cache: CUDA tensors on more than one device")
+            nbytes, ptr = value.numel() * value.element_size(), value.data_ptr()
+            desc.device_sections |= 1 << idx
+        else:
+            value = np.ascontiguousarray(value.cpu().numpy() if hasattr(value, "cpu") else value)
+            nbytes, ptr = value.nbytes, value.ctypes.data
+        if nbytes % _ELEMENT_SIZE[name]:
+            raise NvcError("write_scene_cache: %s holds %d bytes, not a multiple of its %d-byte elements" % (name, nbytes, _ELEMENT_SIZE[name]))
+        keep.append(value)
+        desc.data[idx], desc.count[idx] = (ptr if nbytes else None), nbytes // _ELEMENT_SIZE[name]
+    bound = ctypes.c_size_t()
+    check(lib.nvc_scene_cache_write_bound(ctypes.byref(desc), ctypes.byref(bound)), None, "nvc_scene_cache_write_bound")
+    out = np.empty(max(int(bound.value), 1), np.uint8)
+    size = ctypes.c_size_t()
+    needs_device = desc.device_sections != 0 or (compressed and (desc.count[0] or desc.count[2] or desc.count[4]))
+    if not needs_device:
+        check(lib.nvc_scene_cache_write(None, None, ctypes.byref(desc), out.ctypes.data, out.nbytes, ctypes.byref(size)), None, "nvc_scene_cache_write")
+        return out[: size.value].tobytes()
+    import torch
+
+    dev = torch.device(device) if device is not None else torch.device("cuda", cuda_index if cuda_index is not None else torch.cuda.current_device())
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        ctx = _write_context(lib, dev.index)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        check(lib.nvc_scene_cache_write(ctx, stream, ctypes.byref(desc), out.ctypes.data, out.nbytes, ctypes.byref(size)), ctx, "nvc_scene_cache_write")
+    return out[: size.value].tobytes()
 
 
 def load_scene(path, screen=(1024, 768), depth=None, name=None):
