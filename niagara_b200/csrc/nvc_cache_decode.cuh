@@ -1,6 +1,6 @@
 // nvc_cache_decode.cuh — device decoders of a compressed scene cache's vertex and meshlet streams, for
 // nvc_scene_cache_read_device (nvc_scene_cache_device.cpp).  Their outputs equal the host decoders'
-// (nvc_meshopt_decode.cpp, nvc_scene_cache.cpp) byte for byte; the formats are restated there.
+// (nvc_meshopt_decode.cpp, nvc_scene_cache.cpp) byte for byte; the formats are in nvc_meshopt_format.h.
 //
 // Vertex codec (VERTICES, stride 16; MESHLETVTX0, stride 8).  The host walk (walk_vertex_stream) has already checked the
 // whole stream and found every block's and every byte plane's start, so nothing here can fail.  Three launches:
@@ -14,10 +14,11 @@
 // Meshlet codec (MESHLETDATA).  Each block is a serial chain (triangle history, unseen counter, explicit-byte cursor), so
 // one lane decodes one meshlet.  A warp takes the 32 meshlets after one checkpoint of the host's index: their blocks are
 // adjacent in the stream and are staged in shared memory as one coalesced span when it fits (the reference's 64 / 96
-// meshlets take about 5 KB), else read where they lie.  Every read is bounded by the block's own extent from the size
-// chain, exactly as the host decoder bounds it; a malformed block raises a flag (NVC_ERROR_CORRUPT).  Outputs are whole
-// words: the host index admits only caches whose meshlets' word ranges do not overlap, so a meshlet owns its words, and
-// the zero bytes a word holds past the meshlet's last reference or triangle are what the host's zero fill leaves there.
+// meshlets take about 5 KB), else read where they lie.  Each lane runs the host reader's block decoder
+// (mcodec::decode_block), bounded by the block's own extent from the size chain; a malformed block raises a flag
+// (NVC_ERROR_CORRUPT).  Outputs are whole words: the host index admits only caches whose meshlets' word ranges do not
+// overlap, so a meshlet owns its words, and the zero bytes a word holds past the meshlet's last reference or triangle
+// are what the host's zero fill leaves there.
 #pragma once
 
 #include "nvc_internal.h"
@@ -231,102 +232,42 @@ __global__ void __launch_bounds__(kApplyThreads) decode_vertex_apply_kernel(cons
 		a.out[w] = vcodec::combine(a.carry[w / C / kVertexBlock * C + k], a.out[w], channel);
 }
 
-// One meshlet codec block of `size` bytes -> vertexCount references (whole words, or two uint16 per word with shortRefs)
-// and then triangleCount * 3 index bytes from `out`; false when malformed.  Same reads, checks and order as the host's
-// decodeMeshletBlock.
-__device__ __forceinline__ bool decode_meshlet_block(const uint8_t* block, uint32_t size, uint32_t vertex_count, uint32_t triangle_count, bool short_refs, uint32_t* out)
+// Where mcodec::decode_block puts a meshlet's outputs on the device: whole words from `out` on, the references one per
+// word or, with shortRefs, two per word, then the triangles' index bytes.  `word` holds the `filled` bytes decoded since
+// the last store.
+struct MeshletWordWriter
 {
-	const uint32_t codes_size = (triangle_count + 1) / 2, ctrl_size = (vertex_count + 3) / 4;
-	const uint32_t gap_size = codes_size + ctrl_size < 16 ? 16 - (codes_size + ctrl_size) : 0;
-	if (size < codes_size + ctrl_size + gap_size)
-		return false;
-	const uint8_t* codes = block + size - codes_size;
-	const uint8_t* ctrl = codes - ctrl_size;
-	const uint32_t limit = size - codes_size - ctrl_size - gap_size; // deltas + extra occupy [0, limit)
-	uint32_t cursor = 0;
-
-	uint32_t previous = ~0u, pending = 0;
-	for (uint32_t group = 0; group * 4 < vertex_count; ++group)
-	{
-		const uint32_t control = ctrl[group];
-		for (uint32_t k = 0; k < 4; ++k)
-		{
-			const uint32_t width = control == 0xff ? 4 : (((control >> k) & 1u) | ((control >> (k + 3)) & 2u));
-			if (limit - cursor < width)
-				return false;
-			uint32_t value = 0;
-			for (uint32_t i = 0; i < width; ++i)
-				value |= uint32_t(block[cursor + i]) << (8 * i);
-			cursor += width;
-			previous = previous + ((value >> 1) ^ (0u - (value & 1u))) + 1;
-			const uint32_t i = group * 4 + k;
-			if (i < vertex_count)
-			{
-				if (!short_refs)
-					*out++ = previous;
-				else if (i & 1u)
-					*out++ = pending | (previous << 16);
-				else
-					pending = previous & 0xffffu;
-			}
-		}
-	}
-	if (short_refs && (vertex_count & 1u))
-		*out++ = pending;
-
+	uint32_t* out;
+	bool short_refs;
 	uint32_t word = 0, filled = 0;
-	auto put = [&](uint32_t byte) {
-		word |= byte << (8 * filled);
-		if (++filled == 4)
-		{
-			*out++ = word;
-			word = 0;
-			filled = 0;
-		}
-	};
-	uint32_t h0 = 0, h1 = 0, h2 = 0; // the three previous triangles, a | b << 8 | c << 16, h0 the most recent
-	uint32_t unseen = 0;
-	for (uint32_t t = 0; t < triangle_count; ++t)
+	__device__ __forceinline__ void put(uint32_t value, uint32_t bytes)
 	{
-		const uint32_t code = (codes[t / 2] >> ((t & 1) * 4)) & 15u;
-		uint32_t c[3];
-		if (code < 12)
-		{
-			const uint32_t from = code < 4 ? h0 : code < 8 ? h1 : h2;
-			c[0] = (code & 2) ? from >> 16 : from & 255u;
-			c[1] = (code & 2) ? (from >> 8) & 255u : from >> 16;
-			if (code & 1)
-			{
-				if (cursor >= limit)
-					return false;
-				c[2] = block[cursor++];
-			}
-			else
-				c[2] = unseen++ & 255u;
-		}
-		else
-			for (uint32_t j = 0; j < 3; ++j)
-			{
-				if (code > 12 + j)
-				{
-					if (cursor >= limit)
-						return false;
-					c[j] = block[cursor++];
-				}
-				else
-					c[j] = unseen++ & 255u;
-			}
-		put(c[0]);
-		put(c[1]);
-		put(c[2]);
-		h2 = h1;
-		h1 = h0;
-		h0 = c[0] | (c[1] << 8) | (c[2] << 16);
+		word |= value << (8 * filled);
+		filled += bytes;
+		if (filled == 4)
+			flush();
 	}
-	if (filled)
-		*out = word;
-	return cursor == limit;
-}
+	__device__ __forceinline__ void reference(uint32_t, uint32_t value)
+	{
+		if (short_refs)
+			put(value & 0xffffu, 2);
+		else
+			*out++ = value;
+	}
+	__device__ __forceinline__ void triangle(uint32_t, uint32_t a, uint32_t b, uint32_t c)
+	{
+		put(a, 1);
+		put(b, 1);
+		put(c, 1);
+	}
+	__device__ __forceinline__ void flush()
+	{
+		if (filled)
+			*out++ = word;
+		word = 0;
+		filled = 0;
+	}
+};
 
 __global__ void __launch_bounds__(kMeshletWarps * 32) decode_meshlets_kernel(const MeshletDecodeArgs a)
 {
@@ -361,7 +302,8 @@ __global__ void __launch_bounds__(kMeshletWarps * 32) decode_meshlets_kernel(con
 	const uint32_t at = s_at[warp][lane];
 	const uint32_t size = uint32_t(span[at]) | (uint32_t(span[at + 1]) << 8);
 	const uint2 r = __ldg(reinterpret_cast<const uint2*>(a.records) + first + lane);
-	if (!decode_meshlet_block(span + at + 2, size, r.y & 255u, (r.y >> 8) & 255u, (r.y >> 16) & 1u, a.out + r.x))
+	MeshletWordWriter out = { a.out + r.x, ((r.y >> 16) & 1u) != 0 };
+	if (!mcodec::decode_block(span + at + 2, size, r.y & 255u, (r.y >> 8) & 255u, out))
 		atomicOr(a.corrupt, 1u);
 }
 

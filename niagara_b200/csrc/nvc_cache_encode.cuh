@@ -1,7 +1,7 @@
 // nvc_cache_encode.cuh — device encoders of a compressed scene cache's vertex and meshlet streams, for
 // nvc_scene_cache_write (nvc_scene_cache_write.cpp).  Their output equals, byte for byte, what saveSceneCache writes with
 // meshoptimizer's encoders at the settings it uses (vertex codec v1 at level 2, meshlet codec behind a uint16 size).  The
-// formats are restated in nvc_meshopt_decode.cpp and nvc_scene_cache.cpp; this file restates only the encoder's choices.
+// formats are in nvc_meshopt_format.h and nvc_meshopt_decode.cpp; this file restates only the encoder's choices.
 //
 // Vertex codec.  Both per-stream decisions are made from the input alone, so every 256-vertex block is encoded on its own:
 //   estimate  per 4-byte column, the delta channel (0: per byte, 1: per 16 bits) whose byte planes need fewer bytes on every
@@ -17,9 +17,10 @@
 //             belongs, control bytes first, then the planes in order.  The write pass also stores the header byte and the
 //             tail (zeros up to 24 bytes, vertex 0, the channel bytes).
 // Meshlet codec.  One thread per meshlet, measure then write as above; a meshlet's record is its uint16 size, then the block
-// decode_meshlet_block reads back: the reference deltas, the explicit triangle bytes, the zero gap, the reference control
-// bytes and the triangle codes.  A meshlet whose words lie outside meshletdata or whose counts pass 64 vertices / 96 triangles is not read; it
-// raises a flag that the host turns into NVC_ERROR_INVALID_ARGUMENT before anything reaches the caller's buffer.
+// mcodec::decode_block reads back: the reference deltas, the explicit triangle bytes, the zero gap, the reference control
+// bytes and the triangle codes.  A meshlet whose words lie outside meshletdata or whose counts pass mcodec::kMaxVertices /
+// kMaxTriangles is not read; it raises a flag that the host turns into NVC_ERROR_INVALID_ARGUMENT before anything reaches
+// the caller's buffer.
 #pragma once
 
 #include "nvc_internal.h"
@@ -34,7 +35,6 @@ constexpr uint32_t kEncodeWarps = 4;
 constexpr uint32_t kEstimateThreads = 256;
 constexpr uint32_t kEncodeScanThreads = 1024;
 constexpr uint32_t kMeshletEncodeThreads = 128;
-constexpr uint32_t kMaxMeshletVertices = 64, kMaxMeshletTriangles = 96; // the header's meshletMaxVertices / meshletMaxTriangles
 
 // The delta byte of plane q for a vertex whose words are `cur`, after the vertex whose words are `prev` (C words each):
 // channel 0 zigzags the byte's difference, channel 1 the difference of the 16-bit half holding it.
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(kEncodeScanThreads) encode_scan_kernel(const u
 }
 
 // ---- meshlet codec --------------------------------------------------------------------------------------------------------
-// One meshlet's block, the inverse of decode_meshlet_block (nvc_cache_decode.cuh; layout in nvc_scene_cache.cpp); Write = false
+// One meshlet's block, the inverse of mcodec::decode_block (nvc_meshopt_format.h, with the layout); Write = false
 // only measures.  `out` is where the block starts.  The fixed-size control bytes and codes sit after the variable-size
 // deltas and explicit bytes, so the write pass takes deltas_size / explicit_size from the measure pass.
 template <bool Write>
@@ -347,7 +347,6 @@ __device__ __forceinline__ void encode_meshlet_block(const uint32_t* words, cons
 	const uint32_t vertex_count = m.vertexCount, triangle_count = m.triangleCount;
 	const uint32_t codes_size = (triangle_count + 1) / 2, ctrl_size = (vertex_count + 3) / 4;
 	const uint32_t gap_size = codes_size + ctrl_size < 16 ? 16 - (codes_size + ctrl_size) : 0;
-	const uint32_t ref_words = m.shortRefs ? (vertex_count + 1) / 2 : vertex_count;
 	const uint32_t* refs = words + m.dataOffset;
 	uint8_t* const explicit_bytes = out + deltas_size;
 	uint8_t* const ctrl = explicit_bytes + explicit_size + gap_size;
@@ -400,7 +399,7 @@ __device__ __forceinline__ void encode_meshlet_block(const uint32_t* words, cons
 	// third corner is an explicit byte or the next unseen vertex.  Any other triangle is rotated so that its largest corner
 	// comes last (of equal largest corners, the later one), and codes 12 + e say that its first e corners are explicit bytes
 	// and the rest continue the unseen run.
-	const uint8_t* tris = reinterpret_cast<const uint8_t*>(refs + ref_words);
+	const uint8_t* tris = reinterpret_cast<const uint8_t*>(refs + mcodec::reference_words(vertex_count, m.shortRefs));
 	uint32_t h0 = 0, h1 = 0, h2 = 0; // the three previous triangles as coded, a | b << 8 | c << 16, h0 the most recent
 	uint32_t unseen = 0, explicit_count = 0, code_pair = 0;
 	auto put_explicit = [&](uint32_t v) {
@@ -458,9 +457,8 @@ __device__ __forceinline__ void encode_meshlet_block(const uint32_t* words, cons
 // the meshlet's words lie inside meshletdata and its counts inside the header's limits
 __device__ __forceinline__ bool meshlet_encodable(const NvcMeshlet& m, uint32_t meshletdata_count)
 {
-	const uint64_t ref_words = m.shortRefs ? (uint64_t(m.vertexCount) + 1) / 2 : m.vertexCount;
-	const uint64_t words = ref_words + (uint64_t(m.triangleCount) * 3 + 3) / 4;
-	return m.vertexCount <= kMaxMeshletVertices && m.triangleCount <= kMaxMeshletTriangles && uint64_t(m.dataOffset) + words <= meshletdata_count;
+	return m.vertexCount <= mcodec::kMaxVertices && m.triangleCount <= mcodec::kMaxTriangles &&
+	       uint64_t(m.dataOffset) + mcodec::meshlet_words(m.vertexCount, m.triangleCount, m.shortRefs) <= meshletdata_count;
 }
 
 __device__ __forceinline__ NvcMeshlet load_meshlet(const NvcMeshlet* p)

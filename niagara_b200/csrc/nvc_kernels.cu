@@ -2100,10 +2100,10 @@ __global__ void __launch_bounds__(kRasterWarps * 32) raster_clusters_kernel(cons
 		const uint32_t vertexCount = ml.vertexCount, triangleCount = ml.triangleCount;
 		const uint32_t dataOffset = ml.dataOffset, baseVertex = ml.baseVertex;
 		const bool shortRefs = ml.shortRefs == 1;
-		const uint32_t indexOffset = dataOffset + (shortRefs ? (vertexCount + 1) / 2 : vertexCount);
+		const uint32_t indexOffset = dataOffset + mcodec::reference_words(vertexCount, shortRefs);
 		// the meshlet's references / triangle bytes must lie inside meshletdata (robustBufferAccess in the reference; here: skip)
 		const uint64_t end_words = uint64_t(indexOffset) + (uint64_t(triangleCount) * 3 + 3) / 4;
-		if (vertexCount > 64 || triangleCount > 96 || end_words > p.meshletdata_words)
+		if (vertexCount > mcodec::kMaxVertices || triangleCount > mcodec::kMaxTriangles || end_words > p.meshletdata_words)
 		{
 			rejected += lane == 0;
 			continue;
@@ -2885,7 +2885,7 @@ __global__ void __launch_bounds__(128) cook_pack_kernel(const CookArgs a)
 		hi = mv[i] > hi ? mv[i] : hi;
 	bool short_refs = hi - lo < (1u << 16);
 	uint32_t* dst = a.meshletdata + a.slot_data[s];
-	uint32_t ref_words = short_refs ? (r.z + 1u) / 2u : r.z;
+	const uint32_t ref_words = mcodec::reference_words(r.z, short_refs);
 	for (uint32_t k = 0; k < ref_words; ++k)
 	{
 		if (short_refs)

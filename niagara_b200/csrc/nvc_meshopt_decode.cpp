@@ -14,7 +14,7 @@
 //           v0 {0,2,4,8}, v1 control 0 {0,1,2,4}, control 1 {1,2,4,8}; width 0 = zeros, 8 = 16 literals, else 16 packed
 //           values (1-bit: LSB first, 2/4-bit: MSB first) where the all-ones value means "next escape byte"
 //   deltas per 4-byte group by channel & 3: 0 = per byte zigzag delta, 1 = per 16-bit zigzag delta,
-//           2 = 32-bit xor with the previous value after rotating left by (32 - (channel >> 4)) & 31
+//           2 = 32-bit xor with the previous value after rotating left by (32 - (channel >> 4)) & 31 (vcodec::delta_term)
 //
 // INDEX stream    [0xe0 | version] one code byte per triangle, data bytes, 16-byte aux table at the very end
 //   code < 0xf0 : high nibble = edge FIFO slot (a, b), low nibble = c: 0 next new vertex, 1..12 (v1) / 1..14 (v0)
@@ -95,8 +95,6 @@ bool read_plane(ByteReader& r, int control, int version, uint32_t count, uint8_t
 	});
 }
 
-inline uint32_t rotl(uint32_t v, int r) { return (v << r) | (v >> ((32 - r) & 31)); }
-
 // The parts of a vertex stream around its blocks: the version, the baseline vertex and (v1) the channel bytes in the
 // tail, and the byte range the blocks must fill exactly.
 struct VertexStream
@@ -158,52 +156,16 @@ int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t ver
 			for (int j = 0; j < 4; ++j)
 				if (!read_plane(r, int((ctrl >> (j * 2)) & 3u), version, count, planes[j]))
 					return NVC_ERROR_CORRUPT;
-			int channel = channels ? channels[k / 4] : 0;
-			switch (channel & 3)
-			{
-			case 0:
-				for (int j = 0; j < 4; ++j)
-				{
-					uint8_t p = previous[k + j];
-					for (uint32_t i = 0; i < count; ++i)
-					{
-						uint8_t v = planes[j][i];
-						p = uint8_t(((0u - (v & 1u)) ^ (v >> 1)) + p);
-						block[size_t(i) * stride + k + j] = p;
-					}
-				}
-				break;
-			case 1:
-				for (int half = 0; half < 2; ++half)
-				{
-					uint16_t p = uint16_t(previous[k + half * 2] | (previous[k + half * 2 + 1] << 8));
-					for (uint32_t i = 0; i < count; ++i)
-					{
-						uint16_t v = uint16_t(planes[half * 2][i] | (planes[half * 2 + 1][i] << 8));
-						p = uint16_t(((0u - (v & 1u)) ^ (v >> 1)) + p);
-						block[size_t(i) * stride + k + half * 2] = uint8_t(p);
-						block[size_t(i) * stride + k + half * 2 + 1] = uint8_t(p >> 8);
-					}
-				}
-				break;
-			case 2:
-			{
-				int rot = (32 - (channel >> 4)) & 31;
-				uint32_t p = uint32_t(previous[k]) | (uint32_t(previous[k + 1]) << 8) | (uint32_t(previous[k + 2]) << 16) | (uint32_t(previous[k + 3]) << 24);
-				for (uint32_t i = 0; i < count; ++i)
-				{
-					uint32_t v = uint32_t(planes[0][i]) | (uint32_t(planes[1][i]) << 8) | (uint32_t(planes[2][i]) << 16) | (uint32_t(planes[3][i]) << 24);
-					p = rotl(v, rot) ^ p;
-					uint8_t* dst = block + size_t(i) * stride + k;
-					dst[0] = uint8_t(p);
-					dst[1] = uint8_t(p >> 8);
-					dst[2] = uint8_t(p >> 16);
-					dst[3] = uint8_t(p >> 24);
-				}
-				break;
-			}
-			default:
+			const uint32_t channel = channels ? channels[k / 4] : 0u;
+			if ((channel & 3) == 3) // no delta rule
 				return NVC_ERROR_CORRUPT;
+			uint32_t p;
+			memcpy(&p, previous + k, 4);
+			for (uint32_t i = 0; i < count; ++i)
+			{
+				const uint32_t v = uint32_t(planes[0][i]) | (uint32_t(planes[1][i]) << 8) | (uint32_t(planes[2][i]) << 16) | (uint32_t(planes[3][i]) << 24);
+				p = vcodec::combine(p, vcodec::delta_term(v, channel), channel);
+				memcpy(block + size_t(i) * stride + k, &p, 4);
 			}
 		}
 		memcpy(previous, block + size_t(count - 1) * stride, stride);

@@ -1,7 +1,11 @@
-// nvc_meshopt_format.h — the block structure of the meshopt vertex codec (format restated in nvc_meshopt_decode.cpp),
-// written once for its three users: the host decoder (nvc_meshopt_decode.cpp), the host walk that indexes a stream for
-// the device decoder (same file) and the device decoder (nvc_cache_decode.cuh).  Sizes only come from here, so the walk
-// accepts exactly the streams the host decoder accepts, and the device finds every group where the walk measured it.
+// nvc_meshopt_format.h — the meshopt codec formats, written once for the host and the device.
+//   vertex codec  the block structure (format restated in nvc_meshopt_decode.cpp) and the delta rule, for the host decoder
+//                 and the host walk that indexes a stream for the device decoder (nvc_meshopt_decode.cpp), and the device
+//                 decoder (nvc_cache_decode.cuh).  Sizes only come from here, so the walk accepts exactly the streams the
+//                 host decoder accepts, and the device finds every group where the walk measured it.
+//   meshlet codec a meshlet's words and the block decoder, for the host reader (nvc_scene_cache.cpp), the device decoder
+//                 (nvc_cache_decode.cuh) and the device encoder (nvc_cache_encode.cuh), which writes what it reads back.
+//   index codec   the decoder's FIFO rings, for the host decoder and encoder (nvc_meshopt_decode.cpp, nvc_meshopt_encode.cpp).
 #pragma once
 
 #include <stddef.h>
@@ -127,6 +131,119 @@ NVC_CODEC_FN inline uint32_t combine(uint32_t a, uint32_t b, uint32_t channel)
 }
 
 } // namespace vcodec
+
+// Meshlet codec (meshoptimizer v1.0 meshletcodec, extern/meshoptimizer/src/meshletcodec.cpp — restated, not copied).  A
+// compressed MESHLETDATA section (writeMeshletDataCompressed, scenecache.cpp:84-117) holds, for every Meshlet in order, a
+// uint16 byte count and one block that decodes into the words meshletdata[dataOffset ...]: vertexCount references
+// (uint16 when shortRefs, else uint32) followed by triangleCount * 3 index bytes.
+//
+// Block layout, from the END of the block:   [ deltas | extra | gap | ctrl | codes ]
+//   codes  (triangleCount + 1) / 2 bytes, one nibble per triangle
+//   ctrl   (vertexCount + 3) / 4 bytes, 2 bits per reference (bit k and bit k + 4 of the group's byte)
+//   gap    pads codes + ctrl to 16 bytes (decoder over-read room); deltas and extra must end exactly at the gap
+// References: per group of four, each value is a 0/1/2/3-byte little-endian zigzag delta to the previous
+//   reference plus one (a ctrl byte of 0xff switches the whole group to 4-byte values); the first is relative to -1.
+// Triangles: nibble < 12 re-uses one edge of one of the three previous triangles (nibble / 4 = how far back, bit 1 =
+//   which edge: (a, c) or (c, b)), bit 0 says whether the third corner is an explicit byte or the next unseen
+//   vertex; nibble >= 12 starts a new triangle with nibble - 12 explicit bytes for its (a, b, c) — explicit bytes
+//   come first, then consecutive unseen vertices.
+namespace mcodec
+{
+
+constexpr uint32_t kMaxVertices = 64, kMaxTriangles = 96; // per meshlet, as the reference builds them (the header's meshletMax*)
+
+// words of meshletdata a meshlet's references take (two per word with shortRefs), and all its words with the triangles
+NVC_CODEC_FN inline uint32_t reference_words(uint32_t vertex_count, bool short_refs)
+{
+	return short_refs ? (vertex_count + 1) / 2 : vertex_count;
+}
+
+NVC_CODEC_FN inline uint32_t meshlet_words(uint32_t vertex_count, uint32_t triangle_count, bool short_refs)
+{
+	return reference_words(vertex_count, short_refs) + (triangle_count * 3 + 3) / 4;
+}
+
+// One block of `size` bytes holding vertex_count references and triangle_count triangles; false when malformed.  Every
+// read stays inside the block.  The outputs go to `out`, in this order, as they are decoded:
+//   out.reference(i, value)     each reference, i = 0 .. vertex_count - 1
+//   out.flush()                 after the last reference, and after the last triangle (a writer that assembles whole
+//                               words stores its partial word there)
+//   out.triangle(t, a, b, c)    each triangle, t = 0 .. triangle_count - 1, its corners in the low byte of a, b and c
+template <typename Out>
+NVC_CODEC_FN inline bool decode_block(const uint8_t* block, uint32_t size, uint32_t vertex_count, uint32_t triangle_count, Out& out)
+{
+	const uint32_t codes_size = (triangle_count + 1) / 2, ctrl_size = (vertex_count + 3) / 4;
+	const uint32_t gap_size = codes_size + ctrl_size < 16 ? 16 - (codes_size + ctrl_size) : 0;
+	if (size < codes_size + ctrl_size + gap_size)
+		return false;
+	const uint8_t* codes = block + size - codes_size;
+	const uint8_t* ctrl = codes - ctrl_size;
+	const uint32_t limit = size - codes_size - ctrl_size - gap_size; // deltas + extra occupy [0, limit)
+	uint32_t cursor = 0;
+
+	uint32_t previous = ~0u;
+	for (uint32_t group = 0; group * 4 < vertex_count; ++group)
+	{
+		const uint32_t control = ctrl[group];
+		for (uint32_t k = 0; k < 4; ++k)
+		{
+			const uint32_t width = control == 0xff ? 4 : (((control >> k) & 1u) | ((control >> (k + 3)) & 2u));
+			if (limit - cursor < width)
+				return false;
+			uint32_t value = 0;
+			for (uint32_t i = 0; i < width; ++i)
+				value |= uint32_t(block[cursor + i]) << (8 * i);
+			cursor += width;
+			previous = previous + ((value >> 1) ^ (0u - (value & 1u))) + 1;
+			const uint32_t i = group * 4 + k;
+			if (i < vertex_count)
+				out.reference(i, previous);
+		}
+	}
+	out.flush();
+
+	uint32_t h0 = 0, h1 = 0, h2 = 0; // the three previous triangles, a | b << 8 | c << 16, h0 the most recent
+	uint32_t unseen = 0;
+	for (uint32_t t = 0; t < triangle_count; ++t)
+	{
+		const uint32_t code = (codes[t / 2] >> ((t & 1) * 4)) & 15u;
+		uint32_t c[3];
+		if (code < 12)
+		{
+			const uint32_t from = code < 4 ? h0 : code < 8 ? h1 : h2;
+			c[0] = (code & 2) ? from >> 16 : from & 255u;
+			c[1] = (code & 2) ? (from >> 8) & 255u : from >> 16;
+			if (code & 1)
+			{
+				if (cursor >= limit)
+					return false;
+				c[2] = block[cursor++];
+			}
+			else
+				c[2] = unseen++ & 255u;
+		}
+		else
+			for (uint32_t j = 0; j < 3; ++j)
+			{
+				if (code > 12 + j)
+				{
+					if (cursor >= limit)
+						return false;
+					c[j] = block[cursor++];
+				}
+				else
+					c[j] = unseen++ & 255u;
+			}
+		out.triangle(t, c[0], c[1], c[2]);
+		h2 = h1;
+		h1 = h0;
+		h0 = c[0] | (c[1] << 8) | (c[2] << 16);
+	}
+	out.flush();
+	return cursor == limit;
+}
+
+} // namespace mcodec
 
 namespace icodec
 {

@@ -3,21 +3,8 @@
 // scenecache.cpp:344-353, belongs to the ray-tracing feature and is not applied.)
 //
 // Follows src/scenecache.cpp: SceneHeader (16-55), the section order of saveSceneCache (158-197) and, for the
-// per-meshlet compressed stream, the layout written by writeMeshletDataCompressed (84-117): for every Meshlet, in
-// order, a uint16 byte count followed by one meshopt "meshlet codec" block (meshoptimizer v1.0 meshletcodec,
-// extern/meshoptimizer/src/meshletcodec.cpp) that decodes into the words meshletdata[dataOffset ...]:
-// vertexCount references (uint16 when shortRefs, else uint32) followed by triangleCount * 3 index bytes.
-//
-// Block layout, from the END of the block:   [ deltas | extra | gap | ctrl | codes ]
-//   codes  (triangleCount + 1) / 2 bytes, one nibble per triangle
-//   ctrl   (vertexCount + 3) / 4 bytes, 2 bits per reference (bit k and bit k + 4 of the group's byte)
-//   gap    pads codes + ctrl to 16 bytes (decoder over-read room); deltas and extra must end exactly at the gap
-// References: per group of four, each value is a 0/1/2/3-byte little-endian zigzag delta to the previous
-//   reference plus one (a ctrl byte of 0xff switches the whole group to 4-byte values); the first is relative to -1.
-// Triangles: nibble < 12 re-uses one edge of one of the three previous triangles (nibble / 4 = how far back, bit 1 =
-//   which edge: (a, c) or (c, b)), bit 0 says whether the third corner is an explicit byte or the next unseen
-//   vertex; nibble >= 12 starts a new triangle with nibble - 12 explicit bytes for its (a, b, c) — explicit bytes
-//   come first, then consecutive unseen vertices.
+// per-meshlet compressed stream, the layout written by writeMeshletDataCompressed (84-117), decoded by the meshlet codec of
+// nvc_meshopt_format.h.
 #include "../../include/niagara_cull.h"
 #include "nvc_meshopt_format.h"
 
@@ -26,89 +13,31 @@
 namespace
 {
 
-// one meshlet block -> refs (ref_size 2 or 4 bytes each) and triangles (3 bytes each); false when malformed
-bool decodeMeshletBlock(const uint8_t* block, size_t size, uint32_t vertex_count, uint32_t triangle_count, uint32_t ref_size, uint8_t* refs_out, uint8_t* triangles_out)
+// Where mcodec::decode_block puts a meshlet's outputs on the host: only the bytes of each reference (ref_size 2 or 4)
+// and of each triangle, so that nothing else in the destination changes
+struct MeshletByteWriter
 {
-	size_t codes_size = (triangle_count + 1) / 2, ctrl_size = (vertex_count + 3) / 4;
-	size_t gap_size = codes_size + ctrl_size < 16 ? 16 - (codes_size + ctrl_size) : 0;
-	if (size < codes_size + ctrl_size + gap_size)
-		return false;
-	const uint8_t* codes = block + size - codes_size;
-	const uint8_t* ctrl = codes - ctrl_size;
-	const uint8_t* limit = ctrl - gap_size; // deltas + extra occupy [block, limit)
-	const uint8_t* cursor = block;
-
-	uint32_t previous = ~0u;
-	for (uint32_t group = 0; group * 4 < vertex_count; ++group)
+	uint8_t* refs;
+	uint8_t* triangles;
+	uint32_t ref_size;
+	void reference(uint32_t i, uint32_t value)
 	{
-		uint8_t control = ctrl[group];
-		for (uint32_t k = 0; k < 4; ++k)
+		if (ref_size == 2)
 		{
-			uint32_t width = control == 0xff ? 4 : (((control >> k) & 1u) | ((control >> (k + 3)) & 2u));
-			if (size_t(limit - cursor) < width)
-				return false;
-			uint32_t value = 0;
-			for (uint32_t b = 0; b < width; ++b)
-				value |= uint32_t(cursor[b]) << (8 * b);
-			cursor += width;
-			uint32_t delta = (value >> 1) ^ (0u - (value & 1u));
-			previous = previous + delta + 1;
-			uint32_t i = group * 4 + k;
-			if (i < vertex_count)
-			{
-				if (ref_size == 2)
-				{
-					uint16_t r = uint16_t(previous);
-					memcpy(refs_out + size_t(i) * 2, &r, 2);
-				}
-				else
-					memcpy(refs_out + size_t(i) * 4, &previous, 4);
-			}
-		}
-	}
-
-	struct Tri
-	{
-		uint8_t a, b, c;
-	};
-	Tri history[3] = {}; // [0] = most recent
-	uint32_t unseen = 0;
-	auto corner = [&](bool explicit_byte, uint8_t& out) -> bool {
-		if (explicit_byte)
-		{
-			if (cursor >= limit)
-				return false;
-			out = *cursor++;
+			uint16_t r = uint16_t(value);
+			memcpy(refs + size_t(i) * 2, &r, 2);
 		}
 		else
-			out = uint8_t(unseen++);
-		return true;
-	};
-	for (uint32_t i = 0; i < triangle_count; ++i)
-	{
-		uint32_t code = (codes[i / 2] >> ((i & 1) * 4)) & 0xfu;
-		Tri t;
-		if (code < 12)
-		{
-			const Tri& from = history[code / 4];
-			if (code & 2)
-				t.a = from.c, t.b = from.b;
-			else
-				t.a = from.a, t.b = from.c;
-			if (!corner((code & 1) != 0, t.c))
-				return false;
-		}
-		else if (!corner(code > 12, t.a) || !corner(code > 13, t.b) || !corner(code > 14, t.c))
-			return false;
-		triangles_out[i * 3 + 0] = t.a;
-		triangles_out[i * 3 + 1] = t.b;
-		triangles_out[i * 3 + 2] = t.c;
-		history[2] = history[1];
-		history[1] = history[0];
-		history[0] = t;
+			memcpy(refs + size_t(i) * 4, &value, 4);
 	}
-	return cursor == limit;
-}
+	void triangle(uint32_t t, uint32_t a, uint32_t b, uint32_t c)
+	{
+		triangles[size_t(t) * 3 + 0] = uint8_t(a);
+		triangles[size_t(t) * 3 + 1] = uint8_t(b);
+		triangles[size_t(t) * 3 + 2] = uint8_t(c);
+	}
+	void flush() {}
+};
 
 } // namespace
 
@@ -163,9 +92,7 @@ extern "C" NVC_API int nvc_scene_cache_parse(const void* file, size_t file_size,
 	{
 		NvcMeshlet m;
 		memcpy(&m, meshlets + i, sizeof(m));
-		uint64_t ref_words = m.shortRefs ? (uint64_t(m.vertexCount) + 1) / 2 : m.vertexCount;
-		uint64_t words = ref_words + (uint64_t(m.triangleCount) * 3 + 3) / 4;
-		if (uint64_t(m.dataOffset) + words > h.meshletdataCount)
+		if (uint64_t(m.dataOffset) + nvc::mcodec::meshlet_words(m.vertexCount, m.triangleCount, m.shortRefs) > h.meshletdataCount)
 			return NVC_ERROR_CORRUPT;
 	}
 	if (md.compressed)
@@ -223,10 +150,9 @@ extern "C" NVC_API int nvc_scene_cache_read(const void* file, size_t file_size, 
 		uint16_t n;
 		memcpy(&n, p + at, 2);
 		at += 2;
-		uint32_t ref_words = m.shortRefs ? (uint32_t(m.vertexCount) + 1) / 2 : m.vertexCount;
-		uint8_t* refs = reinterpret_cast<uint8_t*>(words + m.dataOffset);
-		uint8_t* triangles = reinterpret_cast<uint8_t*>(words + m.dataOffset + ref_words);
-		if (!decodeMeshletBlock(p + at, n, m.vertexCount, m.triangleCount, m.shortRefs ? 2u : 4u, refs, triangles))
+		uint32_t* refs = words + m.dataOffset;
+		MeshletByteWriter out = { reinterpret_cast<uint8_t*>(refs), reinterpret_cast<uint8_t*>(refs + nvc::mcodec::reference_words(m.vertexCount, m.shortRefs)), m.shortRefs ? 2u : 4u };
+		if (!nvc::mcodec::decode_block(p + at, n, m.vertexCount, m.triangleCount, out))
 			return NVC_ERROR_CORRUPT;
 		at += n;
 	}
@@ -253,8 +179,7 @@ int index_meshlet_stream(const void* file, size_t file_size, const NvcSceneCache
 	{
 		NvcMeshlet m;
 		memcpy(&m, base + ms.offset + size_t(i) * sizeof(NvcMeshlet), sizeof(m));
-		uint64_t ref_words = m.shortRefs ? (uint64_t(m.vertexCount) + 1) / 2 : m.vertexCount;
-		uint64_t words = ref_words + (uint64_t(m.triangleCount) * 3 + 3) / 4;
+		const uint32_t words = mcodec::meshlet_words(m.vertexCount, m.triangleCount, m.shortRefs);
 		// nvc_scene_cache_parse checks both of these: an info they fail does not describe this file
 		if (uint64_t(m.dataOffset) + words > md.count || at + 2 > md.stored_bytes)
 			return NVC_ERROR_INVALID_ARGUMENT;
@@ -295,6 +220,9 @@ extern "C" NVC_API int nvc_decode_meshlet_stream(void* references, uint32_t vert
 {
 	if (!stream || (reference_size != 2 && reference_size != 4) || vertex_count > 256 || triangle_count > 256 || (!references && vertex_count) || (!triangles && triangle_count))
 		return NVC_ERROR_INVALID_ARGUMENT;
-	return decodeMeshletBlock(static_cast<const uint8_t*>(stream), stream_size, vertex_count, triangle_count, reference_size, static_cast<uint8_t*>(references), triangles) ? NVC_OK
-	                                                                                                                                                                     : NVC_ERROR_CORRUPT;
+	// a block of at most 256 references and 256 triangles spans far less than 4 GiB: a larger stream cannot be one block
+	if (stream_size > 0xffffffffull)
+		return NVC_ERROR_CORRUPT;
+	MeshletByteWriter out = { static_cast<uint8_t*>(references), triangles, reference_size };
+	return nvc::mcodec::decode_block(static_cast<const uint8_t*>(stream), uint32_t(stream_size), vertex_count, triangle_count, out) ? NVC_OK : NVC_ERROR_CORRUPT;
 }

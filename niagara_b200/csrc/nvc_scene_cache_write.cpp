@@ -288,8 +288,8 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 	h.magic = NVC_SCENE_CACHE_MAGIC;
 	h.version = NVC_SCENE_CACHE_VERSION;
 	h.hashMeta = d->hashMeta;
-	h.meshletMaxVertices = 64;
-	h.meshletMaxTriangles = 96;
+	h.meshletMaxVertices = nvc::mcodec::kMaxVertices;
+	h.meshletMaxTriangles = nvc::mcodec::kMaxTriangles;
 	h.clrtMode = uint8_t(d->clrtMode != 0);
 	h.compressed = uint8_t(d->compressed != 0);
 	if (d->compressed)
