@@ -686,8 +686,8 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
  * that always suffice.  NVC_ERROR_INVALID_ARGUMENT: lodCount > 8, an indexCount not a multiple of 3, or a LOD index range or
  * mesh vertex range outside indices / vertices.  Scratch is context-owned and grows as needed, and the call synchronises the
  * device before it enqueues its kernels on `stream`: call it at load time, outside stream capture.  The cooker of clrt
- * builds (a ray-tracing LOD of spatial meshlets, meshletvtx0) is nvc_cook_meshlets_clrt below.  Not covered: the LOD chain
- * itself (meshopt_simplifyWithAttributes: the index ranges are inputs), and appending to existing Meshlet[] / meshletdata. */
+ * builds (a ray-tracing LOD of spatial meshlets, meshletvtx0) is nvc_cook_meshlets_clrt below; the LOD chain that makes the
+ * index ranges is nvc_cook_mesh_lods.  Not covered: appending to existing Meshlet[] / meshletdata. */
 NVC_API int nvc_cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices,
     uint32_t index_count, const NvcMesh* host_meshes, NvcMesh* meshes, uint32_t mesh_count, NvcMeshlet* meshlets, uint32_t meshlet_capacity,
     uint32_t* meshletdata, uint32_t meshletdata_capacity, uint32_t* totals4);
@@ -720,6 +720,34 @@ NVC_API int nvc_cook_meshlets_clrt(NvcContext* ctx, void* stream, const NvcVerte
  * words, and 4 * indexCount meshletvtx0 elements.  NVC_ERROR_INVALID_ARGUMENT when a lodCount > 8. */
 NVC_API int nvc_cook_meshlets_clrt_capacity(const NvcMesh* host_meshes, const float* max_scale, uint32_t mesh_count, uint32_t* meshlets_out,
     uint64_t* words_out, uint64_t* vtx0_out);
+
+/* Builds every mesh's LOD chain on the device, bit-identical to the Mesh[] (meshlet fields aside) and index buffer the reference's
+ * cooker stores (scene.cpp:193-268 appendMesh: meshopt_simplifyWithAttributes with meshopt_SimplifySparse, the decoded normals
+ * as 3 attributes of weight 1 and target error 1e-1, down to 60% of the last LOD's indices, then meshopt_optimizeVertexCache):
+ *   vertices / vertex_count         device: the processed Vertex[] (vb); positions are the fp16 vx, vy, vz, normals np
+ *   lod0_indices / lod0_index_count device: mesh-local LOD 0 indices
+ *   host_meshes / mesh_count        host: vertexOffset, vertexCount and lods[0].indexOffset / indexCount (into lod0_indices) are read
+ *   max_scale                       host, per mesh, as nvc_cook_meshlets_clrt takes it; NULL = 1.0 for every mesh
+ *   meshes                          device out: center / radius (float sum of the dequantised positions over float(vertexCount),
+ *                                   then the largest distance), vertexOffset / vertexCount copied, lodCount, lods[l].indexOffset
+ *                                   (into indices) / indexCount / error, lodRT (the last LOD with error * max_scale < 3e-3, in
+ *                                   every build); every other field 0, meshletOffset / meshletCount included
+ *   indices / index_capacity        device out: the chains, meshes in order and each mesh's LODs in order (the reference's ib)
+ *   totals4                         device out: indices needed (saturated at 2^32 - 1), meshes rejected, overflow flag, 0
+ * A LOD after LOD l is kept when the simplifier returns fewer than 85% of its indices and more than 0; at most 8 LODs.  A mesh
+ * with a LOD 0 index >= its vertexCount is rejected: it gets lodCount 0, contributes no indices, none of its vertices is read,
+ * and it is counted in totals4[1].  When the indices needed exceed index_capacity, totals4[2] is 1 and indices is not written
+ * (meshes is); nvc_cook_mesh_lods_capacity gives a size that always suffices.  NVC_ERROR_INVALID_ARGUMENT: a LOD 0 indexCount
+ * not a multiple of 3, or a LOD 0 index range or mesh vertex range outside lod0_indices / vertices; nothing is written then.
+ * Each mesh's chain runs as one sequential CTA, meshes side by side.  Scratch is context-owned (per mesh about 20 words per
+ * LOD 0 index and 60 per vertex) and grows as needed, and the call synchronises the device before it enqueues its kernels on
+ * `stream`: call it at load time, outside stream capture. */
+NVC_API int nvc_cook_mesh_lods(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* lod0_indices,
+    uint32_t lod0_index_count, const NvcMesh* host_meshes, const float* max_scale, uint32_t mesh_count, NvcMesh* meshes, uint32_t* indices,
+    uint32_t index_capacity, uint32_t* totals4);
+/* Host: the indices nvc_cook_mesh_lods can ever emit for these meshes (saturated at 2^32 - 1): per mesh, the sum over at most 8
+ * LODs of c0 = lods[0].indexCount and c(l+1) = the largest multiple of 3 below size_t(double(c(l)) * 0.85). */
+NVC_API int nvc_cook_mesh_lods_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* indices_out);
 
 #ifdef __cplusplus
 } /* extern "C" */

@@ -2,6 +2,7 @@
 #include "nvc_internal.h"
 #include "nvc_filter.cuh"
 #include "nvc_meshlets.cuh"
+#include "nvc_lods.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -753,16 +754,6 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_meshlet_bounds");
 }
 
-// scene.cpp:266-268: the last LOD with error * maxScale < kShadowLodError (0 when none is), with the reference's float multiply
-static uint32_t lod_rt(const NvcMesh& mesh, float max_scale)
-{
-	uint32_t rt = 0;
-	for (uint32_t i = 0; i < mesh.lodCount; ++i)
-		if (mesh.lods[i].error * max_scale < nvc::cook::kShadowLodError)
-			rt = i;
-	return rt;
-}
-
 NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out)
 {
 	if ((mesh_count && !host_meshes) || !meshlets_out || !words_out)
@@ -808,7 +799,7 @@ static int cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertice
 		const NvcMesh& mesh = host_meshes[i];
 		if (mesh.lodCount > NVC_MAX_LODS || uint64_t(mesh.vertexOffset) + mesh.vertexCount > vertex_count)
 			return NVC_ERROR_INVALID_ARGUMENT;
-		const uint32_t rt = clrt ? lod_rt(mesh, max_scale ? max_scale[i] : 1.0f) : NVC_MAX_LODS;
+		const uint32_t rt = clrt ? nvc::cook::lod_rt(mesh, max_scale ? max_scale[i] : 1.0f) : NVC_MAX_LODS;
 		if (clrt)
 			rt_meshes[i].lodRT = rt;
 		for (uint32_t l = 0; l < mesh.lodCount; ++l)
@@ -950,7 +941,7 @@ NVC_API int nvc_cook_meshlets_clrt_capacity(const NvcMesh* host_meshes, const fl
 	{
 		if (host_meshes[i].lodCount > NVC_MAX_LODS)
 			return NVC_ERROR_INVALID_ARGUMENT;
-		const uint32_t rt = lod_rt(host_meshes[i], max_scale ? max_scale[i] : 1.0f);
+		const uint32_t rt = nvc::cook::lod_rt(host_meshes[i], max_scale ? max_scale[i] : 1.0f);
 		for (uint32_t l = 0; l < host_meshes[i].lodCount; ++l)
 		{
 			const uint32_t n = host_meshes[i].lods[l].indexCount;
@@ -974,3 +965,117 @@ NVC_API int nvc_cook_meshlets_clrt(NvcContext* ctx, void* stream, const NvcVerte
 }
 
 } // extern "C"
+
+// the LOD 0 range and vertex range of every mesh, as nvc_cook_meshlets validates them
+static bool lods_valid(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t vertex_count, uint32_t lod0_index_count)
+{
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		const NvcMesh& mesh = host_meshes[i];
+		if (mesh.lods[0].indexCount % 3 != 0 || uint64_t(mesh.lods[0].indexOffset) + mesh.lods[0].indexCount > lod0_index_count ||
+		    uint64_t(mesh.vertexOffset) + mesh.vertexCount > vertex_count)
+			return false;
+	}
+	return true;
+}
+
+NVC_API int nvc_cook_mesh_lods_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* indices_out)
+{
+	if ((mesh_count && !host_meshes) || !indices_out)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	uint64_t total = 0;
+	for (uint32_t i = 0; i < mesh_count; ++i)
+		total += nvc::lods::chain_capacity(host_meshes[i].lods[0].indexCount);
+	*indices_out = total > 0xffffffffull ? 0xffffffffu : uint32_t(total);
+	return NVC_OK;
+}
+
+NVC_API int nvc_cook_mesh_lods(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* lod0_indices,
+    uint32_t lod0_index_count, const NvcMesh* host_meshes, const float* max_scale, uint32_t mesh_count, NvcMesh* meshes, uint32_t* indices,
+    uint32_t index_capacity, uint32_t* totals4)
+{
+	if (!ctx || !totals4 || (mesh_count && (!host_meshes || !meshes)) || (index_capacity && !indices))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if ((vertex_count && !vertices) || (lod0_index_count && !lod0_indices))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (!lods_valid(host_meshes, mesh_count, vertex_count, lod0_index_count))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+
+	// plan: one job per mesh with its own scratch words (nvc_lods.cuh carve)
+	std::vector<nvc::lods::LodJob> jobs(mesh_count);
+	std::vector<float> scales(mesh_count);
+	uint64_t words = 0;
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		const NvcMesh& mesh = host_meshes[i];
+		nvc::lods::LodJob& job = jobs[i];
+		job.vertex_offset = mesh.vertexOffset;
+		job.vertex_count = mesh.vertexCount;
+		job.index_offset = mesh.lods[0].indexOffset;
+		job.index_count = mesh.lods[0].indexCount;
+		job.scratch = words;
+		job.capacity = nvc::lods::chain_capacity(job.index_count);
+		words += nvc::lods::carve(job.vertex_count, job.index_count, job.capacity, nullptr, nullptr);
+		scales[i] = max_scale ? max_scale[i] : 1.0f;
+	}
+	std::vector<uint32_t> order(mesh_count);
+	for (uint32_t i = 0; i < mesh_count; ++i)
+		order[i] = i;
+	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+
+	size_t bytes = 0;
+	auto take = [&](size_t n) {
+		size_t at = bytes;
+		bytes += (n + 255) & ~size_t(255);
+		return at;
+	};
+	const size_t n = mesh_count;
+	size_t o_jobs = take(n * sizeof(nvc::lods::LodJob)), o_order = take(n * 4), o_scale = take(n * 4);
+	size_t o_chain = take(n * 8), o_base = take(n * 8), o_rejected = take(n), o_words = take(words * 4);
+
+	DeviceGuard guard(ctx->device);
+	// the previous call may still use the scratch, and the copies below are not ordered with `stream`
+	cudaError_t e = cudaDeviceSynchronize();
+	if (e == cudaSuccess && bytes > ctx->cook_scratch_bytes)
+	{
+		cudaFree(ctx->cook_scratch);
+		ctx->cook_scratch = nullptr;
+		ctx->cook_scratch_bytes = 0;
+		e = cudaMalloc(&ctx->cook_scratch, bytes);
+		if (e == cudaErrorMemoryAllocation)
+			return NVC_ERROR_OUT_OF_MEMORY;
+		if (e == cudaSuccess)
+			ctx->cook_scratch_bytes = bytes;
+	}
+	char* base = static_cast<char*>(ctx->cook_scratch);
+	if (e == cudaSuccess && n)
+		e = cudaMemcpy(base + o_jobs, jobs.data(), n * sizeof(nvc::lods::LodJob), cudaMemcpyHostToDevice);
+	if (e == cudaSuccess && n)
+		e = cudaMemcpy(base + o_order, order.data(), n * 4, cudaMemcpyHostToDevice);
+	if (e == cudaSuccess && n)
+		e = cudaMemcpy(base + o_scale, scales.data(), n * 4, cudaMemcpyHostToDevice);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, "nvc_cook_mesh_lods");
+
+	nvc::LodArgs a;
+	a.vertices = vertices;
+	a.lod0_indices = lod0_indices;
+	a.jobs = reinterpret_cast<const nvc::lods::LodJob*>(base + o_jobs);
+	a.order = reinterpret_cast<const uint32_t*>(base + o_order);
+	a.max_scale = reinterpret_cast<const float*>(base + o_scale);
+	a.mesh_count = mesh_count;
+	a.scratch = reinterpret_cast<uint32_t*>(base + o_words);
+	a.chain = reinterpret_cast<uint64_t*>(base + o_chain);
+	a.rejected = reinterpret_cast<uint8_t*>(base + o_rejected);
+	a.base = reinterpret_cast<uint64_t*>(base + o_base);
+	a.meshes = meshes;
+	a.indices = indices;
+	a.index_capacity = index_capacity;
+	a.totals4 = totals4;
+	e = nvc::launch_cook_mesh_lods(a, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_mesh_lods");
+}

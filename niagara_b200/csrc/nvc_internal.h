@@ -275,6 +275,30 @@ struct CookClrtArgs
 	uint32_t meshletvtx0_capacity;
 };
 cudaError_t launch_cook_meshlets_clrt(const CookClrtArgs& c, cudaStream_t stream);
+namespace lods
+{
+struct LodJob;
+}
+// nvc_cook_mesh_lods (nvc_lods.cuh): one job per mesh, in mesh order, and the order the chain kernel takes them in.  Every
+// pointer is device memory.
+struct LodArgs
+{
+	const NvcVertex* vertices;
+	const uint32_t* lod0_indices;
+	const lods::LodJob* jobs;
+	const uint32_t* order;    // mesh indices, largest LOD 0 first
+	const float* max_scale;   // per mesh
+	uint32_t mesh_count;
+	uint32_t* scratch;        // the jobs' scratch words
+	uint64_t* chain;          // per mesh: indices of its chain
+	uint8_t* rejected;        // per mesh
+	uint64_t* base;           // per mesh: first output index
+	NvcMesh* meshes;
+	uint32_t* indices;
+	uint32_t index_capacity;
+	uint32_t* totals4;
+};
+cudaError_t launch_cook_mesh_lods(const LodArgs& a, cudaStream_t stream);
 // nvc_scene_cache_read_device (nvc_cache_decode.cuh).  Every pointer is device memory; `stream` is the section as stored,
 // padded so that word loads that cover its last byte stay inside the allocation.
 struct VertexDecodeArgs

@@ -11,6 +11,7 @@
 #include "nvc_math.cuh"
 #include "nvc_cook.cuh"
 #include "nvc_meshlets.cuh"
+#include "nvc_lods.cuh"
 #include "nvc_tma.cuh"
 #include "nvc_filter.cuh"
 #include "nvc_cache_decode.cuh"
@@ -3395,6 +3396,62 @@ cudaError_t launch_cook_meshlets(const CookArgs& a, cudaStream_t stream)
 	cook_scan_kernel<<<1, kCookScanThreads, 0, stream>>>(a);
 	if (a.slot_count)
 		cook_pack_kernel<<<(a.slot_count + 127u) / 128u, 128, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
+// ---- nvc_cook_mesh_lods: appendMesh's LOD chain (nvc_lods.cuh) ------------------------------------------------------------
+// One single-thread CTA per mesh, largest LOD 0 first: the chain's stages are sequential (each LOD starts from the last one).
+// Writes the Mesh record with chain-relative index offsets and the chain into the mesh's scratch.
+__global__ void __launch_bounds__(1) lods_chain_kernel(const LodArgs a)
+{
+	const uint32_t m = a.order[blockIdx.x];
+	NvcMesh mesh;
+	bool rejected;
+	a.chain[m] = lods::cook_chain(a.jobs[m], a.vertices, a.lod0_indices + a.jobs[m].index_offset, a.max_scale[m], a.scratch, mesh, rejected);
+	a.rejected[m] = rejected;
+	a.meshes[m] = mesh;
+}
+
+// Places the chains in mesh order (the reference's ib layout): offsets, totals, overflow flag.  One thread; a mesh is a
+// few additions.
+__global__ void __launch_bounds__(1) lods_scan_kernel(const LodArgs a)
+{
+	uint64_t base = 0;
+	uint32_t rejected = 0;
+	for (uint32_t m = 0; m < a.mesh_count; ++m)
+	{
+		a.base[m] = base;
+		rejected += a.rejected[m];
+		NvcMesh& mesh = a.meshes[m];
+		for (uint32_t l = 0; l < mesh.lodCount; ++l)
+			mesh.lods[l].indexOffset = uint32_t(base + mesh.lods[l].indexOffset);
+		base += a.chain[m];
+	}
+	a.totals4[0] = base > 0xffffffffull ? 0xffffffffu : uint32_t(base);
+	a.totals4[1] = rejected;
+	a.totals4[2] = base > a.index_capacity;
+	a.totals4[3] = 0;
+}
+
+// Copies each chain to its place, one CTA per mesh; nothing when the chains overflow the capacity
+__global__ void __launch_bounds__(256) lods_copy_kernel(const LodArgs a)
+{
+	if (a.totals4[2])
+		return;
+	const uint32_t m = blockIdx.x;
+	const uint32_t* src = a.scratch + a.jobs[m].scratch;
+	uint32_t* dst = a.indices + a.base[m];
+	for (uint64_t i = threadIdx.x; i < a.chain[m]; i += blockDim.x)
+		dst[i] = src[i];
+}
+
+cudaError_t launch_cook_mesh_lods(const LodArgs& a, cudaStream_t stream)
+{
+	if (a.mesh_count)
+		lods_chain_kernel<<<a.mesh_count, 1, 0, stream>>>(a);
+	lods_scan_kernel<<<1, 1, 0, stream>>>(a);
+	if (a.mesh_count)
+		lods_copy_kernel<<<a.mesh_count, 256, 0, stream>>>(a);
 	return cudaGetLastError();
 }
 

@@ -436,6 +436,17 @@ constexpr float kFillWeight = 0.5f;                           // MESHLET_FILL_WE
 constexpr float kShadowLodError = 3e-3f;                      // scene.cpp:22, the lodRT threshold
 constexpr uint32_t kSpatialLeafSplit = kMaxVertices / 3;      // bvhPackTail's chunk of a vertex-bound run, and bvhSplit's mint
 
+// scene.cpp:266-268, run in every build: the last LOD with error * maxScale < kShadowLodError (0 when none is), with the
+// reference's float multiply
+NVC_HD uint32_t lod_rt(const NvcMesh& mesh, float max_scale)
+{
+	uint32_t rt = 0;
+	for (uint32_t i = 0; i < mesh.lodCount; ++i)
+		if (mesh.lods[i].error * max_scale < kShadowLodError)
+			rt = i;
+	return rt;
+}
+
 // meshopt_buildMeshletsBound(index_count, 64, 24): the meshlet array the reference sizes for every LOD (scene.cpp:98)
 NVC_HD uint64_t spatial_meshlets_bound(uint64_t index_count)
 {

@@ -99,6 +99,13 @@ SIGNATURES = [
          ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p],
     ),
     ("nvc_cook_meshlets_clrt_capacity", ctypes.c_int, [c_void_p, c_void_p, ctypes.c_uint32, c_u32_p, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint64)]),
+    ("nvc_cook_mesh_lods_capacity", ctypes.c_int, [c_void_p, ctypes.c_uint32, c_u32_p]),
+    (
+        "nvc_cook_mesh_lods",
+        ctypes.c_int,
+        [c_void_p, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, c_void_p,
+         ctypes.c_uint32, c_void_p],
+    ),
     ("nvc_nccl_unique_id", ctypes.c_int, [c_void_p]),
     ("nvc_nccl_init", ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int, ctypes.c_int]),
     ("nvc_allgather_visible", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_void_p]),
