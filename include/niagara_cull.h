@@ -519,6 +519,31 @@ NVC_API int nvc_decode_index_stream(uint32_t* dst, uint32_t index_count, const v
 NVC_API int nvc_decode_meshlet_stream(void* references, uint32_t vertex_count, uint32_t reference_size, uint8_t* triangles,
     uint32_t triangle_count, const void* stream, size_t stream_size);
 
+/* The rest of the family a glTF EXT_ / KHR_meshopt_compression buffer view can hold (meshoptimizer's decodeIndexBuffer,
+ * decodeIndexSequence and decodeFilter*):
+ *   index codec            -> dst[index_count] of index_size 2 or 4 bytes, index_count a multiple of 3; 2-byte indices keep
+ *                             the low 16 bits (nvc_decode_index_buffer(dst, n, 4, ...) == nvc_decode_index_stream)
+ *   index-sequence codec   -> dst[index_count] of index_size 2 or 4 bytes (header 0xd0 | version, versions 0 and 1)
+ * Same returns as the stream decoders above.
+ *   vertex filter          in place over count elements of `stride` bytes: OCTAHEDRAL (stride 4 or 8), QUATERNION (8),
+ *                          EXPONENTIAL (any multiple of 4 up to 256), COLOR (4 or 8); NONE leaves the data as it is.
+ *                          NVC_ERROR_INVALID_ARGUMENT for a stride the glTF extension does not allow with the filter.
+ * The filters compute what the reference's SSE2 build computes, operation for operation: float -> int conversions round to
+ * nearest even, and the 8-bit OCTAHEDRAL and COLOR filters use the x86 rsqrtps / rcpps approximations, whose bits the CPU
+ * defines — on x86 the result is bit-identical to the reference's decoder run on the same host (elsewhere those two use the
+ * exact reciprocal square root / reciprocal). */
+typedef enum NvcMeshoptFilter
+{
+	NVC_MESHOPT_FILTER_NONE = 0,
+	NVC_MESHOPT_FILTER_OCTAHEDRAL = 1,
+	NVC_MESHOPT_FILTER_QUATERNION = 2,
+	NVC_MESHOPT_FILTER_EXPONENTIAL = 3,
+	NVC_MESHOPT_FILTER_COLOR = 4
+} NvcMeshoptFilter;
+NVC_API int nvc_decode_index_buffer(void* dst, uint32_t index_count, uint32_t index_size, const void* stream, size_t stream_size);
+NVC_API int nvc_decode_index_sequence(void* dst, uint32_t index_count, uint32_t index_size, const void* stream, size_t stream_size);
+NVC_API int nvc_decode_vertex_filter(int filter, void* data, uint32_t count, uint32_t stride);
+
 /* scene.h:141-161 */
 typedef struct NvcKeyframe
 {
@@ -572,8 +597,16 @@ typedef struct NvcVertex
  * the indexed triangle primitives, materialIndex = material_offset + material, postPass 1 for non-opaque / 2 for transmissive materials),
  * Animation[] + Keyframe[] (LINEAR TRS samplers baked per key through the node hierarchy, scene.cpp:713-830), camera, sun direction,
  * and per primitive the quantised Vertex[] / index arrays of loadVertices (scene.cpp:342-405) — bit-identical to what the reference's
- * importer produces from the same file.  Host only; .gltf (data: URIs or external buffers under base_dir) and .glb.  Sparse accessors
- * and EXT_meshopt_compression: NVC_ERROR_UNSUPPORTED.  Malformed files: NVC_ERROR_CORRUPT, never read outside the buffers. */
+ * importer produces from the same file.  Host only; .gltf (data: URIs or external buffers under base_dir) and .glb.  Sparse accessors:
+ * NVC_ERROR_UNSUPPORTED.  Malformed files: NVC_ERROR_CORRUPT, never read outside the buffers.
+ * Meshopt compression (EXT_meshopt_compression / KHR_meshopt_compression, what gltfpack -c / -cc / -cz writes): every compressed
+ * buffer view is validated as cgltf_validate does and decoded at import, used by a primitive or not (the reference's
+ * decompressMeshopt, scene.cpp:405-470); the decoded bytes are what accessors and animation samplers read.  A buffer without data
+ * is accepted when it is a meshopt fallback buffer ("fallback": true); an uncompressed view into one is NVC_ERROR_CORRUPT.  A
+ * view that breaks a validation rule is NVC_ERROR_CORRUPT; a stream that does not decode returns the decoder's status
+ * (NVC_ERROR_CORRUPT, or NVC_ERROR_UNSUPPORTED for a newer codec version); NVC_ERROR_OUT_OF_MEMORY when a decoded view cannot be
+ * allocated.  Filters follow nvc_decode_vertex_filter (bit-identical
+ * to the reference on an x86 host). */
 typedef struct NvcGltfScene NvcGltfScene;
 typedef struct NvcGltfInfo
 {

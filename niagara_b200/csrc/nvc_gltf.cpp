@@ -11,8 +11,18 @@
 // _world (extern/cgltf/cgltf.h:2137-2216), decomposeTransform is scene.cpp:295-340.  Host code, strict IEEE
 // (-ffp-contract=off).  Supported: .gltf with data: URIs or external buffers, .glb; dense accessors of every component
 // type; TRS or matrix nodes; KHR_materials_transmission (presence), KHR_lights_punctual (directional -> sun, point -> light
-// slots for animation targets).  Not supported (NVC_ERROR_UNSUPPORTED): sparse accessors, EXT_meshopt_compression.
+// slots for animation targets), EXT_meshopt_compression / KHR_meshopt_compression (below).  Not supported
+// (NVC_ERROR_UNSUPPORTED): sparse accessors.
+//
+// Meshopt compression, as loadScene's decompressMeshopt (scene.cpp:405-470) runs it after cgltf_validate: every buffer view
+// with the extension (buffer, byteOffset, byteLength, byteStride, count, mode, filter; cgltf.h:5045-5130, both extension
+// names parse alike) is checked against cgltf_validate's rules (cgltf.h:1640-1667) and decoded at import, whether a used
+// primitive reads it or not, with the decoders of nvc_meshopt_host.h (inline, so that this file links on its own).  The
+// decoded bytes replace the view's contents for every accessor.  A buffer without data is accepted when it declares itself a
+// meshopt fallback buffer ("fallback": true: gltfpack writes the compressed views' uncompressed size there and no bytes);
+// an uncompressed view into it is refused.
 #include "../../include/niagara_cull.h"
+#include "nvc_meshopt_host.h"
 
 #include <ctype.h>
 #include <math.h>
@@ -24,6 +34,7 @@
 #include <algorithm>
 #include <map>
 #include <memory>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -339,7 +350,9 @@ struct Sampler
 
 struct NvcGltfScene
 {
-	std::vector<std::vector<uint8_t>> buffers;
+	std::vector<std::vector<uint8_t>> buffers; // the file's buffers, then one per decoded meshopt view
+	std::vector<uint64_t> buffer_length;       // byteLength as declared (what cgltf_validate checks views against)
+	std::vector<bool> buffer_fallback;         // a meshopt fallback buffer: no data
 	std::vector<BufferView> views;
 	std::vector<Accessor> accessors;
 	std::vector<std::vector<Primitive>> meshes;
@@ -633,6 +646,141 @@ bool parse_float_array(const Json* j, float* out, size_t n)
 	return true;
 }
 
+// ---- EXT_meshopt_compression / KHR_meshopt_compression ---------------------------------------------------------------------
+bool is_meshopt_fallback(const Json& buffer)
+{
+	const Json* ext = buffer.get("extensions");
+	for (const char* name : { "EXT_meshopt_compression", "KHR_meshopt_compression" })
+		if (const Json* e = ext ? ext->get(name) : nullptr)
+			if (const Json* f = e->get("fallback"))
+				if (f->type == Json::Bool && f->b)
+					return true;
+	return false;
+}
+
+const Json* meshopt_extension(const Json& view)
+{
+	const Json* ext = view.get("extensions");
+	if (!ext)
+		return nullptr;
+	if (const Json* e = ext->get("EXT_meshopt_compression"))
+		return e;
+	return ext->get("KHR_meshopt_compression");
+}
+
+enum MeshoptMode
+{
+	kModeInvalid,
+	kModeAttributes,
+	kModeTriangles,
+	kModeIndices
+};
+
+struct MeshoptView
+{
+	size_t buffer = 0;
+	uint64_t offset = 0, length = 0, stride = 0, count = 0;
+	int mode = kModeInvalid;
+	int filter = nvc::kFilterNone;
+};
+
+uint64_t num_u64(const Json* j)
+{
+	// a negative value fails every range check below, as cgltf's conversion to cgltf_size makes it huge
+	return j && j->is_number() ? uint64_t((long long)(j->num)) : 0;
+}
+
+// the extension's fields (cgltf.h:5045-5130: a missing or unknown mode is invalid, an unknown filter is NONE) checked against
+// cgltf_validate (cgltf.h:1640-1667), all sizes in 64 bits
+int parse_meshopt_view(NvcGltfScene* s, const Json& e, const BufferView& outer, MeshoptView& m)
+{
+	const long long buffer = num_i(e.get("buffer"), -1);
+	m.offset = num_u64(e.get("byteOffset"));
+	m.length = num_u64(e.get("byteLength"));
+	m.stride = num_u64(e.get("byteStride"));
+	m.count = num_u64(e.get("count"));
+	const Json* mode = e.get("mode");
+	const std::string ms = mode && mode->type == Json::String ? mode->str : "";
+	m.mode = ms == "ATTRIBUTES" ? kModeAttributes : ms == "TRIANGLES" ? kModeTriangles : ms == "INDICES" ? kModeIndices : kModeInvalid;
+	const Json* filter = e.get("filter");
+	const std::string fs = filter && filter->type == Json::String ? filter->str : "";
+	m.filter = fs == "OCTAHEDRAL" ? nvc::kFilterOctahedral : fs == "QUATERNION" ? nvc::kFilterQuaternion : fs == "EXPONENTIAL" ? nvc::kFilterExponential : fs == "COLOR" ? nvc::kFilterColor : nvc::kFilterNone;
+	if (buffer < 0 || size_t(buffer) >= s->buffers.size() || s->buffer_fallback[size_t(buffer)])
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt source buffer missing or without data");
+	m.buffer = size_t(buffer);
+	const uint64_t size = s->buffer_length[m.buffer];
+	if (m.length > size || m.offset > size - m.length)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt source outside its buffer");
+	if (outer.stride && outer.stride != m.stride)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt byteStride differs from the bufferView's");
+	if ((m.count && m.stride > UINT64_MAX / m.count) || outer.length != m.stride * m.count)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt byteStride * count differs from the bufferView's byteLength");
+	if (m.mode == kModeInvalid)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt mode");
+	if (m.mode == kModeAttributes && !(m.stride % 4 == 0 && m.stride <= 256))
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt ATTRIBUTES stride");
+	if (m.mode == kModeTriangles && m.count % 3 != 0)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt TRIANGLES count");
+	if (m.mode != kModeAttributes && m.stride != 2 && m.stride != 4)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt index stride");
+	if (m.mode != kModeAttributes && m.filter != nvc::kFilterNone)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt filter on an index view");
+	if ((m.filter == nvc::kFilterOctahedral || m.filter == nvc::kFilterColor) && m.stride != 4 && m.stride != 8)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt filter stride");
+	if (m.filter == nvc::kFilterQuaternion && m.stride != 8)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt filter stride");
+	return NVC_OK;
+}
+
+// decodes one validated view into a buffer of its own and points the view at it
+int decode_meshopt_view(NvcGltfScene* s, const MeshoptView& m, BufferView& view)
+{
+	const uint8_t* source = s->buffers[m.buffer].data() + m.offset;
+	const size_t length = size_t(m.length);
+	// every stream spends bytes in proportion to what it decodes (v1 vertex blocks at least their control bytes, index
+	// streams a byte per triangle / index): a count the source cannot hold fails to decode, so it is refused before the
+	// output is allocated
+	uint64_t least = 0;
+	if (m.mode == kModeAttributes)
+	{
+		const uint64_t per_block = m.stride ? nvc::vcodec::block_vertices(uint32_t(m.stride)) : 1;
+		least = (m.count + per_block - 1) / per_block * (m.stride / 4);
+	}
+	else
+		least = m.mode == kModeTriangles ? m.count / 3 : m.count;
+	if (m.mode == kModeAttributes && m.stride == 0)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt ATTRIBUTES stride 0");
+	if (m.count > 0xffffffffull || least > m.length)
+		return fail(s, NVC_ERROR_CORRUPT, "meshopt count larger than its stream can hold");
+	std::vector<uint8_t> out;
+	try
+	{
+		out.resize(size_t(m.stride * m.count));
+	}
+	catch (const std::bad_alloc&)
+	{
+		return fail(s, NVC_ERROR_OUT_OF_MEMORY, "meshopt view");
+	}
+	const uint32_t count = uint32_t(m.count), stride = uint32_t(m.stride);
+	int status = NVC_OK;
+	if (m.mode == kModeAttributes)
+		status = nvc::decode_vertex_stream(source, length, count, stride, out.data());
+	else if (m.mode == kModeTriangles)
+		status = nvc::decode_index_buffer(source, length, count, stride, out.data());
+	else
+		status = nvc::decode_index_sequence(source, length, count, stride, out.data());
+	if (status != NVC_OK)
+		return fail(s, status, "meshopt stream does not decode");
+	nvc::decode_vertex_filter(m.filter, out.data(), count, stride);
+	view.buffer = s->buffers.size();
+	view.offset = 0;
+	view.length = out.size();
+	s->buffers.push_back(std::move(out));
+	s->buffer_length.push_back(view.length);
+	s->buffer_fallback.push_back(false);
+	return NVC_OK;
+}
+
 int build(NvcGltfScene* s, const Json& root, const uint8_t* glb_bin, size_t glb_bin_size, const char* base_dir, uint32_t first_mesh_index, uint32_t material_offset)
 {
 	auto arr = [&](const char* key) -> const Json* {
@@ -645,6 +793,7 @@ int build(NvcGltfScene* s, const Json& root, const uint8_t* glb_bin, size_t glb_
 		{
 			const Json& b = a->at(i);
 			std::vector<uint8_t> data;
+			bool fallback = false;
 			const Json* uri = b.get("uri");
 			if (uri && uri->type == Json::String)
 			{
@@ -676,30 +825,52 @@ int build(NvcGltfScene* s, const Json& root, const uint8_t* glb_bin, size_t glb_
 			}
 			else if (i == 0 && glb_bin)
 				data.assign(glb_bin, glb_bin + glb_bin_size);
+			else if (is_meshopt_fallback(b))
+				fallback = true;
 			else
 				return fail(s, NVC_ERROR_CORRUPT, "buffer without data");
 			const long long want = num_i(b.get("byteLength"), -1);
-			if (want < 0 || size_t(want) > data.size())
+			if (want < 0 || (!fallback && size_t(want) > data.size()))
 				return fail(s, NVC_ERROR_CORRUPT, "buffer shorter than byteLength");
 			s->buffers.push_back(std::move(data));
+			s->buffer_length.push_back(uint64_t(want));
+			s->buffer_fallback.push_back(fallback);
 		}
 	// ---- buffer views / accessors ----
+	std::vector<std::pair<size_t, MeshoptView>> compressed; // view index, its extension
 	if (const Json* a = arr("bufferViews"))
 		for (size_t i = 0; i < a->size(); ++i)
 		{
 			const Json& v = a->at(i);
-			if (const Json* ext = v.get("extensions"))
-				if (ext->get("EXT_meshopt_compression"))
-					return fail(s, NVC_ERROR_UNSUPPORTED, "EXT_meshopt_compression is not supported");
 			BufferView bv;
 			bv.buffer = size_t(num_i(v.get("buffer"), 0));
 			bv.offset = size_t(num_i(v.get("byteOffset"), 0));
 			bv.length = size_t(num_i(v.get("byteLength"), 0));
 			bv.stride = size_t(num_i(v.get("byteStride"), 0));
-			if (bv.buffer >= s->buffers.size() || uint64_t(bv.offset) + bv.length > s->buffers[bv.buffer].size())
+			const Json* mc = meshopt_extension(v);
+			// a fallback buffer has no bytes: its declared length bounds the views that a decoded stream will replace
+			const uint64_t room = bv.buffer >= s->buffers.size() ? 0 : s->buffer_fallback[bv.buffer] ? s->buffer_length[bv.buffer] : s->buffers[bv.buffer].size();
+			if (bv.buffer >= s->buffers.size() || bv.length > room || bv.offset > room - bv.length)
 				return fail(s, NVC_ERROR_CORRUPT, "bufferView outside its buffer");
+			if (s->buffer_fallback[bv.buffer] && !mc)
+				return fail(s, NVC_ERROR_CORRUPT, "uncompressed bufferView in a meshopt fallback buffer");
+			if (mc)
+			{
+				MeshoptView m;
+				int status = parse_meshopt_view(s, *mc, bv, m);
+				if (status != NVC_OK)
+					return status;
+				compressed.emplace_back(i, m);
+			}
 			s->views.push_back(bv);
 		}
+	// decompressMeshopt: every compressed view, used or not, before any accessor is read
+	for (const auto& c : compressed)
+	{
+		int status = decode_meshopt_view(s, c.second, s->views[c.first]);
+		if (status != NVC_OK)
+			return status;
+	}
 	if (const Json* a = arr("accessors"))
 		for (size_t i = 0; i < a->size(); ++i)
 		{

@@ -1,11 +1,11 @@
 // nvc_meshopt_format.h — the meshopt codec formats, written once for the host and the device.
-//   vertex codec  the block structure (format restated in nvc_meshopt_decode.cpp) and the delta rule, for the host decoder
-//                 and the host walk that indexes a stream for the device decoder (nvc_meshopt_decode.cpp), and the device
+//   vertex codec  the block structure (format restated in nvc_meshopt_host.h) and the delta rule, for the host decoder
+//                 and the host walk that indexes a stream for the device decoder (nvc_meshopt_host.h), and the device
 //                 decoder (nvc_cache_decode.cuh).  Sizes only come from here, so the walk accepts exactly the streams the
 //                 host decoder accepts, and the device finds every group where the walk measured it.
 //   meshlet codec a meshlet's words and the block decoder, for the host reader (nvc_scene_cache.cpp), the device decoder
 //                 (nvc_cache_decode.cuh) and the device encoder (nvc_cache_encode.cuh), which writes what it reads back.
-//   index codec   the decoder's FIFO rings, for the host decoder and encoder (nvc_meshopt_decode.cpp, nvc_meshopt_encode.cpp).
+//   index codec   the decoder's FIFO rings, for the host decoder and encoder (nvc_meshopt_host.h, nvc_meshopt_encode.cpp).
 #pragma once
 
 #include <stddef.h>
@@ -275,11 +275,7 @@ struct VertexStreamTail
 	const uint8_t* channels;
 };
 
-// nvc_meshopt_decode.cpp (host)
-int decode_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint8_t* out);
-int decode_index_stream(const uint8_t* stream, size_t stream_size, uint32_t index_count, uint32_t* out);
-int walk_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_t vertex_count, uint32_t stride, uint32_t* block_start, uint16_t* plane_offset,
-    VertexStreamTail* tail);
+// the host decoders (decode_vertex_stream, walk_vertex_stream, decode_index_stream, ...) are inline in nvc_meshopt_host.h
 
 // nvc_meshopt_encode.cpp (host): index codec v1 of index_count indices (a multiple of 3) into out[index_stream_bound]
 size_t index_stream_bound(size_t index_count);

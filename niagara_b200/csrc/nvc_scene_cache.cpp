@@ -1,12 +1,12 @@
 // nvc_scene_cache.cpp — reader of the reference's scene cache (.cache v7), SURVEY §8(f) row N2.  Host only.
-// (The vertex / index codec streams are decoded by nvc_meshopt_decode.cpp; loadSceneCache's normalizeIndicesForOMM step,
+// (The vertex / index codec streams are decoded by nvc_meshopt_host.h; loadSceneCache's normalizeIndicesForOMM step,
 // scenecache.cpp:344-353, belongs to the ray-tracing feature and is not applied.)
 //
 // Follows src/scenecache.cpp: SceneHeader (16-55), the section order of saveSceneCache (158-197) and, for the
 // per-meshlet compressed stream, the layout written by writeMeshletDataCompressed (84-117), decoded by the meshlet codec of
 // nvc_meshopt_format.h.
 #include "../../include/niagara_cull.h"
-#include "nvc_meshopt_format.h"
+#include "nvc_meshopt_host.h"
 
 #include <string.h>
 

@@ -3,7 +3,7 @@
 // (walk_vertex_stream, index_meshlet_stream), and are decoded by the kernels of nvc_cache_decode.cuh.  Raw sections are
 // copied up; INDICES is decoded on the host (the index codec is one sequential FIFO state machine) and copied up.
 #include "nvc_internal.h"
-#include "nvc_meshopt_format.h"
+#include "nvc_meshopt_host.h"
 
 #include <string.h>
 

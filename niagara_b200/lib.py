@@ -79,6 +79,9 @@ SIGNATURES = [
     ("nvc_decode_vertex_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_index_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
     ("nvc_decode_meshlet_stream", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
+    ("nvc_decode_index_buffer", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
+    ("nvc_decode_index_sequence", ctypes.c_int, [c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p, ctypes.c_size_t]),
+    ("nvc_decode_vertex_filter", ctypes.c_int, [ctypes.c_int, c_void_p, ctypes.c_uint32, ctypes.c_uint32]),
     (
         "nvc_host_animate",
         ctypes.c_int,

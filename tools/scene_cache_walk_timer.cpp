@@ -2,7 +2,7 @@
 // index_meshlet_stream over MESHLETDATA, the serial part of the device read.  Built from the library's host sources by
 // tools/scene_cache_device_bench.py.  Usage: scene_cache_walk_timer <file.cache> <iterations>; prints one JSON line with
 // the median milliseconds of each walk.
-#include "nvc_meshopt_format.h"
+#include "nvc_meshopt_host.h"
 
 #include <algorithm>
 #include <chrono>
