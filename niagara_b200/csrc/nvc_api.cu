@@ -18,12 +18,8 @@ namespace
 // 48 KB a kernel gets without opting in; its static part is 8.2 KB (s_stage[8][256] + barriers), so 39 KB = 9984 texels.
 constexpr uint32_t kMaxStageTexels = 9984;
 
-int cuda_fail(NvcContext* ctx, cudaError_t e, const char* what)
-{
-	if (ctx)
-		ctx->last_error = std::string(what) + ": " + cudaGetErrorString(e);
-	return NVC_ERROR_CUDA;
-}
+using nvc::cuda_fail;
+using nvc::device_is_current;
 
 // Picks the coarse tail of the pyramid that is staged into shared memory by TMA: the largest set of top mips whose
 // texels fit the budget, whose start is 16-byte aligned in the packed allocation and that holds at least one 16-byte unit.
@@ -78,19 +74,6 @@ struct DeviceGuard
 			cudaSetDevice(previous);
 	}
 };
-
-// Pass calls launch on the caller's stream, which lives on the context's device: that device must be current
-// (the reference drives one VkDevice from one thread; nothing here switches devices behind the caller's back).
-bool device_is_current(NvcContext* ctx)
-{
-	int current = -1;
-	if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
-	{
-		ctx->last_error = "the context's CUDA device is not the calling thread's current device";
-		return false;
-	}
-	return true;
-}
 
 bool fill_hiz(const NvcHiZ* in, nvc::HiZDesc& out)
 {
@@ -249,10 +232,8 @@ NVC_API void nvc_destroy(NvcContext* ctx)
 		cudaFree(ctx->meshlet_cone);
 	if (ctx->hiz_fp)
 		cudaFree(ctx->hiz_fp);
-	if (ctx->cook_scratch)
-		cudaFree(ctx->cook_scratch);
-	if (ctx->cache_scratch)
-		cudaFree(ctx->cache_scratch);
+	if (ctx->load_scratch)
+		cudaFree(ctx->load_scratch);
 	delete ctx;
 }
 
@@ -754,23 +735,69 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_meshlet_bounds");
 }
 
+} // extern "C"
+
+namespace
+{
+
+// The meshlet cooker's walk over meshes x LODs, in mesh then LOD order: per LOD its job (the scratch ranges of
+// nvc_cook_meshlets laid out in that order) and whether it is the mesh's lodRT, and the sums of the per-LOD bounds.  The
+// capacity queries return the sums and the cook plans its call with the jobs, so that a capacity is what the call plans.
+struct CookPlan
+{
+	std::vector<nvc::cook::CookJob> jobs;
+	std::vector<uint32_t> job_rt;  // per job: 1 for the mesh's lodRT
+	std::vector<uint32_t> mesh_rt; // per mesh: its lodRT (clrt), NVC_MAX_LODS otherwise
+	uint64_t tri = 0, vtx = 0, idx = 0;
+	uint64_t slots = 0, words = 0, vtx0 = 0; // meshlet slots (= the meshlet bound), meshletdata words, meshletvtx0 elements
+	bool in_range = true; // every vertex range and LOD index range inside the call's buffers, index counts multiples of 3
+};
+
+// false: a mesh has more than NVC_MAX_LODS LODs.  Without clrt no LOD is a lodRT (greedy bounds throughout).
+bool plan_cook(const NvcMesh* meshes, uint32_t mesh_count, bool clrt, const float* max_scale, uint64_t vertex_count, uint64_t index_count, CookPlan& plan)
+{
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		const NvcMesh& mesh = meshes[i];
+		if (mesh.lodCount > NVC_MAX_LODS)
+			return false;
+		plan.in_range = plan.in_range && uint64_t(mesh.vertexOffset) + mesh.vertexCount <= vertex_count;
+		const uint32_t rt = clrt ? nvc::cook::lod_rt(mesh, max_scale ? max_scale[i] : 1.0f) : NVC_MAX_LODS;
+		plan.mesh_rt.push_back(rt);
+		for (uint32_t l = 0; l < mesh.lodCount; ++l)
+		{
+			const NvcMeshLod& lod = mesh.lods[l];
+			const uint32_t n = lod.indexCount;
+			plan.in_range = plan.in_range && n % 3 == 0 && uint64_t(lod.indexOffset) + n <= index_count;
+			plan.jobs.push_back({ i, l, lod.indexOffset, n, mesh.vertexOffset, mesh.vertexCount, plan.tri, plan.vtx, plan.idx, plan.slots });
+			plan.job_rt.push_back(l == rt);
+			plan.tri += n / 3;
+			plan.vtx += mesh.vertexCount;
+			plan.idx += n;
+			plan.slots += l == rt ? nvc::cook::spatial_meshlets_bound(n) : nvc::cook::meshlets_bound(n);
+			plan.words += l == rt ? nvc::cook::spatial_words_bound(n) : nvc::cook::words_bound(n);
+			plan.vtx0 += l == rt ? 4ull * n : 0ull;
+		}
+	}
+	return true;
+}
+
+uint32_t saturate32(uint64_t v)
+{
+	return v > 0xffffffffull ? 0xffffffffu : uint32_t(v);
+}
+
+} // namespace
+
 NVC_API int nvc_cook_meshlets_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* meshlets_out, uint64_t* words_out)
 {
 	if ((mesh_count && !host_meshes) || !meshlets_out || !words_out)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	uint64_t meshlets = 0, words = 0;
-	for (uint32_t i = 0; i < mesh_count; ++i)
-	{
-		if (host_meshes[i].lodCount > NVC_MAX_LODS)
-			return NVC_ERROR_INVALID_ARGUMENT;
-		for (uint32_t l = 0; l < host_meshes[i].lodCount; ++l)
-		{
-			meshlets += nvc::cook::meshlets_bound(host_meshes[i].lods[l].indexCount);
-			words += nvc::cook::words_bound(host_meshes[i].lods[l].indexCount);
-		}
-	}
-	*meshlets_out = meshlets > 0xffffffffull ? 0xffffffffu : uint32_t(meshlets);
-	*words_out = words;
+	CookPlan plan; // the capacity does not depend on the ranges
+	if (!plan_cook(host_meshes, mesh_count, false, nullptr, 0, 0, plan))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	*meshlets_out = saturate32(plan.slots);
+	*words_out = plan.words;
 	return NVC_OK;
 }
 
@@ -786,94 +813,54 @@ static int cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertice
 	if (!device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 
-	// plan: one job per LOD in mesh then LOD order, each with its own scratch ranges
-	std::vector<nvc::cook::CookJob> jobs;
-	std::vector<uint32_t> job_rt;
+	CookPlan plan;
+	if (!plan_cook(host_meshes, mesh_count, clrt, max_scale, vertex_count, index_count, plan) || !plan.in_range)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if ((plan.idx && !indices) || (plan.jobs.size() && !vertices))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (plan.slots > 0xffffffffull)
+		return NVC_ERROR_INVALID_ARGUMENT; // meshlet slots are counted in 32 bits
+	const std::vector<nvc::cook::CookJob>& jobs = plan.jobs;
+	const uint32_t job_count = uint32_t(jobs.size());
+	const uint64_t tri = plan.tri, vtx = plan.vtx, idx = plan.idx, slot = plan.slots;
 	// clrt: Mesh[] as uploaded, with lodRT set
 	std::vector<NvcMesh> rt_meshes;
-	if (clrt && mesh_count)
-		rt_meshes.assign(host_meshes, host_meshes + mesh_count);
-	uint64_t tri = 0, vtx = 0, idx = 0, slot = 0;
-	for (uint32_t i = 0; i < mesh_count; ++i)
-	{
-		const NvcMesh& mesh = host_meshes[i];
-		if (mesh.lodCount > NVC_MAX_LODS || uint64_t(mesh.vertexOffset) + mesh.vertexCount > vertex_count)
-			return NVC_ERROR_INVALID_ARGUMENT;
-		const uint32_t rt = clrt ? nvc::cook::lod_rt(mesh, max_scale ? max_scale[i] : 1.0f) : NVC_MAX_LODS;
-		if (clrt)
-			rt_meshes[i].lodRT = rt;
-		for (uint32_t l = 0; l < mesh.lodCount; ++l)
+	if (clrt)
+		for (uint32_t i = 0; i < mesh_count; ++i)
 		{
-			const NvcMeshLod& lod = mesh.lods[l];
-			if (lod.indexCount % 3 != 0 || uint64_t(lod.indexOffset) + lod.indexCount > index_count)
-				return NVC_ERROR_INVALID_ARGUMENT;
-			if (lod.indexCount && !indices)
-				return NVC_ERROR_INVALID_ARGUMENT;
-			nvc::cook::CookJob job = { i, l, lod.indexOffset, lod.indexCount, mesh.vertexOffset, mesh.vertexCount, tri, vtx, idx, slot };
-			jobs.push_back(job);
-			job_rt.push_back(l == rt);
-			tri += lod.indexCount / 3;
-			vtx += mesh.vertexCount;
-			idx += lod.indexCount;
-			slot += l == rt ? nvc::cook::spatial_meshlets_bound(lod.indexCount) : nvc::cook::meshlets_bound(lod.indexCount);
+			rt_meshes.push_back(host_meshes[i]);
+			rt_meshes[i].lodRT = plan.mesh_rt[i];
 		}
-	}
-	if (jobs.size() && !vertices)
-		return NVC_ERROR_INVALID_ARGUMENT;
-	if (slot > 0xffffffffull)
-		return NVC_ERROR_INVALID_ARGUMENT; // meshlet slots are counted in 32 bits
-	const uint32_t job_count = uint32_t(jobs.size());
 	// the longest jobs start first; outputs are placed by job index, so the order does not change them.  clrt: the greedy
 	// jobs, then the ray-tracing jobs, each longest first
 	std::vector<uint32_t> order(job_count);
 	for (uint32_t j = 0; j < job_count; ++j)
 		order[j] = j;
 	auto longer = [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; };
-	auto rt_end = std::stable_partition(order.begin(), order.end(), [&](uint32_t x) { return !job_rt[x]; });
+	auto rt_end = std::stable_partition(order.begin(), order.end(), [&](uint32_t x) { return !plan.job_rt[x]; });
 	std::stable_sort(order.begin(), rt_end, longer);
 	std::stable_sort(rt_end, order.end(), longer);
 	const uint32_t greedy_count = uint32_t(rt_end - order.begin());
 
-	// scratch layout, 256-byte aligned sub-allocations
-	size_t bytes = 0;
-	auto take = [&](size_t n) {
-		size_t at = bytes;
-		bytes += (n + 255) & ~size_t(255);
-		return at;
-	};
-	size_t o_jobs = take(job_count * sizeof(nvc::cook::CookJob)), o_order = take(job_count * 4ull);
-	size_t o_cones = take(tri * 24u), o_counts = take(vtx * 4u), o_offsets = take(vtx * 4u), o_used = take(vtx * 2u);
-	size_t o_data = take(idx * 4u), o_mlv = take(idx * 4u), o_mlt = take(idx), o_emitted = take(tri);
-	size_t o_nodes = take(tri * 24u), o_kdi = take(tri * 4u), o_records = take(slot * 16u);
-	size_t o_words = take(slot * 4u), o_min = take(slot * 4u), o_sdata = take(slot * 4u);
-	size_t o_jm = take(job_count * 4ull), o_jf = take(job_count * 4ull);
-	size_t o_rt = take(clrt ? job_count * 4ull : 0), o_svtx = take(clrt ? slot * 4u : 0);
+	nvc::ScratchPlan sp;
+	const size_t o_jobs = sp.take(job_count * sizeof(nvc::cook::CookJob)), o_order = sp.take(job_count * 4ull);
+	const size_t o_cones = sp.take(tri * 24u), o_counts = sp.take(vtx * 4u), o_offsets = sp.take(vtx * 4u), o_used = sp.take(vtx * 2u);
+	const size_t o_data = sp.take(idx * 4u), o_mlv = sp.take(idx * 4u), o_mlt = sp.take(idx), o_emitted = sp.take(tri);
+	const size_t o_nodes = sp.take(tri * 24u), o_kdi = sp.take(tri * 4u), o_records = sp.take(slot * 16u);
+	const size_t o_words = sp.take(slot * 4u), o_min = sp.take(slot * 4u), o_sdata = sp.take(slot * 4u);
+	const size_t o_jm = sp.take(job_count * 4ull), o_jf = sp.take(job_count * 4ull);
+	const size_t o_rt = clrt ? sp.take(job_count * 4ull) : 0, o_svtx = clrt ? sp.take(slot * 4u) : 0;
 
-	DeviceGuard guard(ctx->device);
-	// the previous call may still use the scratch, and the copies below are not ordered with `stream`
+	// the previous user of the scratch finishes first
 	cudaError_t e = cudaDeviceSynchronize();
-	if (e == cudaSuccess && bytes > ctx->cook_scratch_bytes)
-	{
-		cudaFree(ctx->cook_scratch);
-		ctx->cook_scratch = nullptr;
-		ctx->cook_scratch_bytes = 0;
-		e = cudaMalloc(&ctx->cook_scratch, bytes);
-		if (e == cudaErrorMemoryAllocation)
-			return NVC_ERROR_OUT_OF_MEMORY;
-		if (e == cudaSuccess)
-			ctx->cook_scratch_bytes = bytes;
-	}
-	char* base = static_cast<char*>(ctx->cook_scratch);
-	if (e == cudaSuccess && job_count)
-		e = cudaMemcpy(base + o_jobs, jobs.data(), job_count * sizeof(nvc::cook::CookJob), cudaMemcpyHostToDevice);
-	if (e == cudaSuccess && job_count)
-		e = cudaMemcpy(base + o_order, order.data(), job_count * 4ull, cudaMemcpyHostToDevice);
-	if (e == cudaSuccess && clrt && job_count)
-		e = cudaMemcpy(base + o_rt, job_rt.data(), job_count * 4ull, cudaMemcpyHostToDevice);
-	if (e == cudaSuccess && mesh_count)
-		e = cudaMemcpy(meshes, clrt ? rt_meshes.data() : host_meshes, size_t(mesh_count) * sizeof(NvcMesh), cudaMemcpyHostToDevice);
-	if (e == cudaSuccess)
-		e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, what);
+	e = nvc::reserve_scratch(ctx, sp.bytes);
+	if (e != cudaSuccess)
+		return nvc::load_fail(ctx, e, what);
+	char* base = static_cast<char*>(ctx->load_scratch);
+	e = nvc::upload({ { base + o_jobs, jobs.data(), job_count * sizeof(nvc::cook::CookJob) }, { base + o_order, order.data(), job_count * 4ull },
+	    { base + o_rt, plan.job_rt.data(), clrt ? job_count * 4ull : 0 }, { meshes, clrt ? rt_meshes.data() : host_meshes, size_t(mesh_count) * sizeof(NvcMesh) } });
 	if (e != cudaSuccess)
 		return cuda_fail(ctx, e, what);
 
@@ -936,23 +923,12 @@ NVC_API int nvc_cook_meshlets_clrt_capacity(const NvcMesh* host_meshes, const fl
 {
 	if ((mesh_count && !host_meshes) || !meshlets_out || !words_out || !vtx0_out)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	uint64_t meshlets = 0, words = 0, vtx0 = 0;
-	for (uint32_t i = 0; i < mesh_count; ++i)
-	{
-		if (host_meshes[i].lodCount > NVC_MAX_LODS)
-			return NVC_ERROR_INVALID_ARGUMENT;
-		const uint32_t rt = nvc::cook::lod_rt(host_meshes[i], max_scale ? max_scale[i] : 1.0f);
-		for (uint32_t l = 0; l < host_meshes[i].lodCount; ++l)
-		{
-			const uint32_t n = host_meshes[i].lods[l].indexCount;
-			meshlets += l == rt ? nvc::cook::spatial_meshlets_bound(n) : nvc::cook::meshlets_bound(n);
-			words += l == rt ? nvc::cook::spatial_words_bound(n) : nvc::cook::words_bound(n);
-			vtx0 += l == rt ? 4ull * n : 0ull;
-		}
-	}
-	*meshlets_out = meshlets > 0xffffffffull ? 0xffffffffu : uint32_t(meshlets);
-	*words_out = words;
-	*vtx0_out = vtx0;
+	CookPlan plan;
+	if (!plan_cook(host_meshes, mesh_count, true, max_scale, 0, 0, plan))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	*meshlets_out = saturate32(plan.slots);
+	*words_out = plan.words;
+	*vtx0_out = plan.vtx0;
 	return NVC_OK;
 }
 
@@ -964,29 +940,48 @@ NVC_API int nvc_cook_meshlets_clrt(NvcContext* ctx, void* stream, const NvcVerte
 	    meshletdata_capacity, totals8, true, max_scale, meshletvtx0, meshletvtx0_capacity, "nvc_cook_meshlets_clrt");
 }
 
-} // extern "C"
-
-// the LOD 0 range and vertex range of every mesh, as nvc_cook_meshlets validates them
-static bool lods_valid(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t vertex_count, uint32_t lod0_index_count)
+namespace
 {
+
+// The LOD cooker's walk over the meshes: per mesh its job, with its own scratch words (nvc_lods.cuh carve), and the sums of
+// the chain capacities and scratch words.  The capacity query returns the first sum; nvc_cook_mesh_lods plans its call with
+// the jobs.
+struct LodPlan
+{
+	std::vector<nvc::lods::LodJob> jobs;
+	uint64_t indices = 0, words = 0;
+	bool in_range = true; // every LOD 0 and vertex range inside the call's buffers, LOD 0 index counts multiples of 3
+};
+
+LodPlan plan_lods(const NvcMesh* meshes, uint32_t mesh_count, uint64_t vertex_count, uint64_t lod0_index_count)
+{
+	LodPlan plan;
+	plan.jobs.resize(mesh_count);
 	for (uint32_t i = 0; i < mesh_count; ++i)
 	{
-		const NvcMesh& mesh = host_meshes[i];
-		if (mesh.lods[0].indexCount % 3 != 0 || uint64_t(mesh.lods[0].indexOffset) + mesh.lods[0].indexCount > lod0_index_count ||
-		    uint64_t(mesh.vertexOffset) + mesh.vertexCount > vertex_count)
-			return false;
+		const NvcMesh& mesh = meshes[i];
+		nvc::lods::LodJob& job = plan.jobs[i];
+		job.vertex_offset = mesh.vertexOffset;
+		job.vertex_count = mesh.vertexCount;
+		job.index_offset = mesh.lods[0].indexOffset;
+		job.index_count = mesh.lods[0].indexCount;
+		job.scratch = plan.words;
+		job.capacity = nvc::lods::chain_capacity(job.index_count);
+		plan.words += nvc::lods::carve(job.vertex_count, job.index_count, job.capacity, nullptr, nullptr);
+		plan.indices += job.capacity;
+		plan.in_range = plan.in_range && job.index_count % 3 == 0 && uint64_t(job.index_offset) + job.index_count <= lod0_index_count &&
+		                uint64_t(job.vertex_offset) + job.vertex_count <= vertex_count;
 	}
-	return true;
+	return plan;
 }
+
+} // namespace
 
 NVC_API int nvc_cook_mesh_lods_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* indices_out)
 {
 	if ((mesh_count && !host_meshes) || !indices_out)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	uint64_t total = 0;
-	for (uint32_t i = 0; i < mesh_count; ++i)
-		total += nvc::lods::chain_capacity(host_meshes[i].lods[0].indexCount);
-	*indices_out = total > 0xffffffffull ? 0xffffffffu : uint32_t(total);
+	*indices_out = saturate32(plan_lods(host_meshes, mesh_count, 0, 0).indices); // the capacity does not depend on the ranges
 	return NVC_OK;
 }
 
@@ -998,66 +993,35 @@ NVC_API int nvc_cook_mesh_lods(NvcContext* ctx, void* stream, const NvcVertex* v
 		return NVC_ERROR_INVALID_ARGUMENT;
 	if ((vertex_count && !vertices) || (lod0_index_count && !lod0_indices))
 		return NVC_ERROR_INVALID_ARGUMENT;
-	if (!lods_valid(host_meshes, mesh_count, vertex_count, lod0_index_count))
+	const LodPlan plan = plan_lods(host_meshes, mesh_count, vertex_count, lod0_index_count);
+	if (!plan.in_range)
 		return NVC_ERROR_INVALID_ARGUMENT;
 	if (!device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 
-	// plan: one job per mesh with its own scratch words (nvc_lods.cuh carve)
-	std::vector<nvc::lods::LodJob> jobs(mesh_count);
-	std::vector<float> scales(mesh_count);
-	uint64_t words = 0;
-	for (uint32_t i = 0; i < mesh_count; ++i)
-	{
-		const NvcMesh& mesh = host_meshes[i];
-		nvc::lods::LodJob& job = jobs[i];
-		job.vertex_offset = mesh.vertexOffset;
-		job.vertex_count = mesh.vertexCount;
-		job.index_offset = mesh.lods[0].indexOffset;
-		job.index_count = mesh.lods[0].indexCount;
-		job.scratch = words;
-		job.capacity = nvc::lods::chain_capacity(job.index_count);
-		words += nvc::lods::carve(job.vertex_count, job.index_count, job.capacity, nullptr, nullptr);
-		scales[i] = max_scale ? max_scale[i] : 1.0f;
-	}
+	const std::vector<nvc::lods::LodJob>& jobs = plan.jobs;
+	std::vector<float> scales(mesh_count, 1.0f);
+	if (max_scale)
+		scales.assign(max_scale, max_scale + mesh_count);
 	std::vector<uint32_t> order(mesh_count);
 	for (uint32_t i = 0; i < mesh_count; ++i)
 		order[i] = i;
 	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
 
-	size_t bytes = 0;
-	auto take = [&](size_t n) {
-		size_t at = bytes;
-		bytes += (n + 255) & ~size_t(255);
-		return at;
-	};
 	const size_t n = mesh_count;
-	size_t o_jobs = take(n * sizeof(nvc::lods::LodJob)), o_order = take(n * 4), o_scale = take(n * 4);
-	size_t o_chain = take(n * 8), o_base = take(n * 8), o_rejected = take(n), o_words = take(words * 4);
+	nvc::ScratchPlan sp;
+	const size_t o_jobs = sp.take(n * sizeof(nvc::lods::LodJob)), o_order = sp.take(n * 4), o_scale = sp.take(n * 4);
+	const size_t o_chain = sp.take(n * 8), o_base = sp.take(n * 8), o_rejected = sp.take(n), o_words = sp.take(plan.words * 4);
 
-	DeviceGuard guard(ctx->device);
-	// the previous call may still use the scratch, and the copies below are not ordered with `stream`
+	// the previous user of the scratch finishes first
 	cudaError_t e = cudaDeviceSynchronize();
-	if (e == cudaSuccess && bytes > ctx->cook_scratch_bytes)
-	{
-		cudaFree(ctx->cook_scratch);
-		ctx->cook_scratch = nullptr;
-		ctx->cook_scratch_bytes = 0;
-		e = cudaMalloc(&ctx->cook_scratch, bytes);
-		if (e == cudaErrorMemoryAllocation)
-			return NVC_ERROR_OUT_OF_MEMORY;
-		if (e == cudaSuccess)
-			ctx->cook_scratch_bytes = bytes;
-	}
-	char* base = static_cast<char*>(ctx->cook_scratch);
-	if (e == cudaSuccess && n)
-		e = cudaMemcpy(base + o_jobs, jobs.data(), n * sizeof(nvc::lods::LodJob), cudaMemcpyHostToDevice);
-	if (e == cudaSuccess && n)
-		e = cudaMemcpy(base + o_order, order.data(), n * 4, cudaMemcpyHostToDevice);
-	if (e == cudaSuccess && n)
-		e = cudaMemcpy(base + o_scale, scales.data(), n * 4, cudaMemcpyHostToDevice);
-	if (e == cudaSuccess)
-		e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, "nvc_cook_mesh_lods");
+	e = nvc::reserve_scratch(ctx, sp.bytes);
+	if (e != cudaSuccess)
+		return nvc::load_fail(ctx, e, "nvc_cook_mesh_lods");
+	char* base = static_cast<char*>(ctx->load_scratch);
+	e = nvc::upload({ { base + o_jobs, jobs.data(), n * sizeof(nvc::lods::LodJob) }, { base + o_order, order.data(), n * 4 }, { base + o_scale, scales.data(), n * 4 } });
 	if (e != cudaSuccess)
 		return cuda_fail(ctx, e, "nvc_cook_mesh_lods");
 

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <initializer_list>
 #include <string>
 
 #include "../../include/niagara_cull.h"
@@ -46,12 +47,11 @@ struct NvcContext
 	uint32_t hiz_fp_first = 0; // first mip with a footprint image (env NVC_FP_FIRST_LEVEL)
 	uint32_t hiz_fp_offset[NVC_MAX_HIZ_LEVELS] = {};
 	bool hiz_fp_valid = false; // set by nvc_depth_pyramid, cleared by nvc_prepare_hiz
-	// nvc_cook_meshlets: job table and per-job scratch, grown as needed
-	void* cook_scratch = nullptr;
-	size_t cook_scratch_bytes = 0;
-	// nvc_scene_cache_read_device: the staged stream and its index; nvc_scene_cache_write: the inputs and encoded streams; grown as needed
-	void* cache_scratch = nullptr;
-	size_t cache_scratch_bytes = 0;
+	// the load-time calls' scratch, grown as needed (nvc::reserve_scratch): the cookers' job tables and per-job arrays, the
+	// staged streams of nvc_scene_cache_read_device, the inputs and encoded streams of nvc_scene_cache_write.  Each of these
+	// calls synchronises the device before it touches it, so one call's use has ended when the next one's begins.
+	void* load_scratch = nullptr;
+	size_t load_scratch_bytes = 0;
 };
 
 namespace nvc
@@ -60,6 +60,34 @@ void nccl_destroy(NvcContext* ctx);   // nvc_nccl.cpp
 void gather_destroy(NvcContext* ctx); // nvc_peer.cu
 uint32_t* gather_fused_target(NvcContext* ctx);
 uint32_t gather_reserved_blocks(NvcContext* ctx); // nvc_peer.cu: CTA slots the persistent cluster grid leaves to the exchange's kernels // nvc_peer.cu: multicast destination of the armed late drawcull, or nullptr (disarms)
+
+// Calls that work on the caller's stream need the context's device to be current (the reference drives one VkDevice from
+// one thread; nothing here switches devices behind the caller's back).
+inline bool device_is_current(NvcContext* ctx)
+{
+	int current = -1;
+	if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
+	{
+		ctx->last_error = "the context's CUDA device is not the calling thread's current device";
+		return false;
+	}
+	return true;
+}
+
+// A failed CUDA step of the call `what`, named with the error in nvc_last_error: NVC_ERROR_CUDA
+inline int cuda_fail(NvcContext* ctx, cudaError_t e, const char* what)
+{
+	if (ctx)
+		ctx->last_error = std::string(what) + ": " + cudaGetErrorString(e);
+	return NVC_ERROR_CUDA;
+}
+// as cuda_fail, but a failed allocation is NVC_ERROR_OUT_OF_MEMORY: the scene-cache calls' steps, and the cookers' growth of
+// the load-time scratch
+inline int load_fail(NvcContext* ctx, cudaError_t e, const char* what)
+{
+	cuda_fail(ctx, e, what);
+	return e == cudaErrorMemoryAllocation ? NVC_ERROR_OUT_OF_MEMORY : NVC_ERROR_CUDA;
+}
 
 // Device-side counters owned by the context.  Each pass's last-block epilogue leaves them zeroed, which replaces
 // the reference's vkCmdFillBuffer resets (niagara.cpp:1541,1586) and keeps every pass a single launch.
@@ -323,7 +351,7 @@ struct MeshletDecodeArgs
 	uint32_t* corrupt; // set to 1 by a malformed block
 };
 cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stream);
-// Sub-allocations of the context's cache scratch (nvc_scene_cache_read_device, nvc_scene_cache_write), each 256-byte aligned
+// Sub-allocations of the context's load-time scratch, each 256-byte aligned; `bytes` ends where the last one does
 struct ScratchPlan
 {
 	size_t bytes = 0;
@@ -334,18 +362,38 @@ struct ScratchPlan
 		return at;
 	}
 };
-// grows the context's cache scratch to `bytes`; its previous user has finished (the caller synchronised the device)
-inline cudaError_t reserve_cache_scratch(NvcContext* ctx, size_t bytes)
+// grows the context's load-time scratch to `bytes`; its previous user has finished (the caller synchronised the device)
+inline cudaError_t reserve_scratch(NvcContext* ctx, size_t bytes)
 {
-	if (bytes <= ctx->cache_scratch_bytes)
+	if (bytes <= ctx->load_scratch_bytes)
 		return cudaSuccess;
-	cudaFree(ctx->cache_scratch);
-	ctx->cache_scratch = nullptr;
-	ctx->cache_scratch_bytes = 0;
-	cudaError_t e = cudaMalloc(&ctx->cache_scratch, bytes);
+	cudaFree(ctx->load_scratch);
+	ctx->load_scratch = nullptr;
+	ctx->load_scratch_bytes = 0;
+	cudaError_t e = cudaMalloc(&ctx->load_scratch, bytes);
 	if (e == cudaSuccess)
-		ctx->cache_scratch_bytes = bytes;
+		ctx->load_scratch_bytes = bytes;
 	return e;
+}
+// One host-to-device copy of a load-time call; a copy of 0 bytes is skipped.
+struct Upload
+{
+	void* dst;
+	const void* src;
+	size_t bytes;
+};
+// A copy from pageable host memory may return before its DMA has landed, and it is not ordered with a non-blocking stream:
+// the copies are followed by a device synchronise, before a kernel reads them or the call returns.
+inline cudaError_t upload(std::initializer_list<Upload> copies)
+{
+	for (const Upload& c : copies)
+		if (c.bytes)
+		{
+			cudaError_t e = cudaMemcpy(c.dst, c.src, c.bytes, cudaMemcpyHostToDevice);
+			if (e != cudaSuccess)
+				return e;
+		}
+	return cudaDeviceSynchronize();
 }
 // nvc_scene_cache_write (nvc_cache_encode.cuh).  Every pointer is device memory.
 constexpr uint32_t kVertexBlockEncode = 256; // vcodec::block_vertices of strides 8 and 16

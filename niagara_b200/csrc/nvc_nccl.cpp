@@ -133,14 +133,8 @@ NVC_API int nvc_allgather_visible(NvcContext* ctx, void* stream, const void* loc
 		ctx->last_error = "nvc_nccl_init has not been called";
 		return NVC_ERROR_NCCL;
 	}
-	{
-		int current = -1;
-		if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
-		{
-			ctx->last_error = "the context's CUDA device is not the calling thread's current device";
-			return NVC_ERROR_INVALID_ARGUMENT;
-		}
-	}
+	if (!nvc::device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
 	ncclComm_t comm = static_cast<ncclComm_t>(ctx->nccl_comm);
 	cudaStream_t s = static_cast<cudaStream_t>(stream);
 	// one fused group: the 16-byte counter blocks and the fixed-capacity slabs

@@ -388,17 +388,6 @@ NVC_API int nvc_gather_connect(NvcContext* ctx, const void* all_tickets /* world
 	return NVC_OK;
 }
 
-static bool on_context_device(NvcContext* ctx)
-{
-	int current = -1;
-	if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
-	{
-		ctx->last_error = "the context's CUDA device is not the calling thread's current device";
-		return false;
-	}
-	return true;
-}
-
 // Enqueues (after everything already on `stream`): push of local_slab / local_count4 into slot `rank` of every rank's
 // gathered buffers (parity of the new frame tag) over the side streams, then the flag raise.  Returns immediately;
 // `stream` itself is not blocked by the copies (call nvc_gather_wait on the stream that consumes the gathered data).
@@ -408,7 +397,7 @@ NVC_API int nvc_gather_push(NvcContext* ctx, void* stream, const void* local_sla
 	NvcGather* g = ctx ? static_cast<NvcGather*>(ctx->gather) : nullptr;
 	if (!g || !g->connected || !local_slab || !local_count4)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	if (!on_context_device(ctx))
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	cudaStream_t s = static_cast<cudaStream_t>(stream);
 	// fused mode: the tag was taken (and the peers' acknowledgements awaited) by nvc_gather_fuse_next_drawcull, and the slab
@@ -505,7 +494,7 @@ NVC_API int nvc_gather_wait(NvcContext* ctx, void* stream)
 	NvcGather* g = ctx ? static_cast<NvcGather*>(ctx->gather) : nullptr;
 	if (!g || !g->connected)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	if (!on_context_device(ctx))
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	cudaStream_t s = static_cast<cudaStream_t>(stream);
 	cudaError_t e = cudaSuccess;
@@ -571,7 +560,7 @@ NVC_API int nvc_gather_attach(NvcContext* ctx, size_t slab_bytes, int rank, int 
 	for (int p = 0; p < world; ++p)
 		if (!peer_regions[p] || (reinterpret_cast<uintptr_t>(peer_regions[p]) & 15u))
 			return NVC_ERROR_INVALID_ARGUMENT;
-	if (!on_context_device(ctx))
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	nvc::gather_destroy(ctx);
 	NvcGather* g = new NvcGather();
@@ -654,7 +643,7 @@ NVC_API int nvc_gather_fuse_next_drawcull(NvcContext* ctx, void* stream)
 	NvcGather* g = ctx ? static_cast<NvcGather*>(ctx->gather) : nullptr;
 	if (!g || !g->connected || g->mode != 3 || !g->mc_slabs)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	if (!on_context_device(ctx))
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	if (g->fused_tag != 0)
 	{
@@ -687,7 +676,7 @@ NVC_API int nvc_gather_graph_advance(NvcContext* ctx, void* stream, uint32_t fra
 	NvcGather* g = ctx ? static_cast<NvcGather*>(ctx->gather) : nullptr;
 	if (!g || !g->connected || frames == 0 || (frames & 1u))
 		return NVC_ERROR_INVALID_ARGUMENT;
-	if (!on_context_device(ctx))
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	advance_epoch_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(g->count_stage + 8, frames);
 	cudaError_t e = cudaGetLastError();
@@ -705,7 +694,7 @@ NVC_API int nvc_gather_status(NvcContext* ctx, int* timed_out)
 	NvcGather* g = ctx ? static_cast<NvcGather*>(ctx->gather) : nullptr;
 	if (!g || !timed_out)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	if (!on_context_device(ctx))
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
 	uint32_t v = 0;
 	cudaError_t e = cudaMemcpy(&v, g->count_stage + 9, sizeof(v), cudaMemcpyDeviceToHost);

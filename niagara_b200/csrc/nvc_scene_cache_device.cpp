@@ -12,23 +12,10 @@
 namespace
 {
 
-int cuda_fail(NvcContext* ctx, cudaError_t e)
-{
-	ctx->last_error = std::string("nvc_scene_cache_read_device: ") + cudaGetErrorString(e);
-	return e == cudaErrorMemoryAllocation ? NVC_ERROR_OUT_OF_MEMORY : NVC_ERROR_CUDA;
-}
-
 // a stored stream staged in whole words: the kernels' word loads cover its last byte and go no further
 size_t staged_bytes(uint64_t stored)
 {
 	return size_t((stored + 3) & ~uint64_t(3));
-}
-
-// A copy from pageable host memory may return before its DMA has landed, and it is not ordered with a non-blocking
-// `stream`: callers synchronise the device after their uploads, before a kernel reads them or the call returns.
-cudaError_t upload(void* dst, const void* src, size_t n)
-{
-	return n ? cudaMemcpy(dst, src, n, cudaMemcpyHostToDevice) : cudaSuccess;
 }
 
 int read_vertices(NvcContext* ctx, cudaStream_t stream, const uint8_t* data, const NvcSceneCacheSection& sec, uint32_t vertex_count, uint32_t stride, void* dst)
@@ -44,18 +31,13 @@ int read_vertices(NvcContext* ctx, cudaStream_t stream, const uint8_t* data, con
 	nvc::ScratchPlan plan; // the staged stream is taken last: a scratch allocated for this call ends where its last word does
 	const size_t o_start = plan.take(block_start.size() * 4), o_plane = plan.take(plane_offset.size() * 2);
 	const size_t o_carry = plan.take(size_t(blocks) * stride), o_stream = plan.take(staged_bytes(sec.stored_bytes));
-	cudaError_t e = nvc::reserve_cache_scratch(ctx, plan.bytes);
-	char* base = static_cast<char*>(ctx->cache_scratch);
+	cudaError_t e = nvc::reserve_scratch(ctx, plan.bytes);
+	char* base = static_cast<char*>(ctx->load_scratch);
 	if (e == cudaSuccess)
-		e = upload(base + o_stream, data, sec.stored_bytes);
-	if (e == cudaSuccess)
-		e = upload(base + o_start, block_start.data(), block_start.size() * 4);
-	if (e == cudaSuccess)
-		e = upload(base + o_plane, plane_offset.data(), plane_offset.size() * 2);
-	if (e == cudaSuccess)
-		e = cudaDeviceSynchronize();
+		e = nvc::upload({ { base + o_stream, data, sec.stored_bytes }, { base + o_start, block_start.data(), block_start.size() * 4 },
+		    { base + o_plane, plane_offset.data(), plane_offset.size() * 2 } });
 	if (e != cudaSuccess)
-		return cuda_fail(ctx, e);
+		return nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 
 	nvc::VertexDecodeArgs a;
 	memset(&a, 0, sizeof(a));
@@ -73,7 +55,7 @@ int read_vertices(NvcContext* ctx, cudaStream_t stream, const uint8_t* data, con
 	e = nvc::launch_decode_vertices(a, stride, stream);
 	if (e == cudaSuccess)
 		e = cudaDeviceSynchronize();
-	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e);
+	return e == cudaSuccess ? NVC_OK : nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 }
 
 int read_meshletdata(NvcContext* ctx, cudaStream_t stream, const void* file, size_t file_size, const NvcSceneCacheInfo* info, void* dst)
@@ -89,23 +71,18 @@ int read_meshletdata(NvcContext* ctx, cudaStream_t stream, const void* file, siz
 	nvc::ScratchPlan plan;
 	const size_t o_check = plan.take(checkpoints.size() * 4), o_records = plan.take(records.size() * 4), o_flag = plan.take(4);
 	const size_t o_stream = plan.take(staged_bytes(sec.stored_bytes));
-	cudaError_t e = nvc::reserve_cache_scratch(ctx, plan.bytes);
-	char* base = static_cast<char*>(ctx->cache_scratch);
+	cudaError_t e = nvc::reserve_scratch(ctx, plan.bytes);
+	char* base = static_cast<char*>(ctx->load_scratch);
 	if (e == cudaSuccess)
-		e = upload(base + o_stream, static_cast<const uint8_t*>(file) + sec.offset, sec.stored_bytes);
-	if (e == cudaSuccess)
-		e = upload(base + o_check, checkpoints.data(), checkpoints.size() * 4);
-	if (e == cudaSuccess)
-		e = upload(base + o_records, records.data(), records.size() * 4);
-	if (e == cudaSuccess)
-		e = cudaDeviceSynchronize();
+		e = nvc::upload({ { base + o_stream, static_cast<const uint8_t*>(file) + sec.offset, sec.stored_bytes }, { base + o_check, checkpoints.data(), checkpoints.size() * 4 },
+		    { base + o_records, records.data(), records.size() * 4 } });
 	// as the host read: bytes no meshlet writes (padding, the unused half of an odd shortRefs word) are 0
 	if (e == cudaSuccess && sec.decoded_bytes)
 		e = cudaMemsetAsync(dst, 0, sec.decoded_bytes, stream);
 	if (e == cudaSuccess)
 		e = cudaMemsetAsync(base + o_flag, 0, 4, stream);
 	if (e != cudaSuccess)
-		return cuda_fail(ctx, e);
+		return nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 
 	nvc::MeshletDecodeArgs a;
 	a.stream = reinterpret_cast<const uint8_t*>(base + o_stream);
@@ -121,7 +98,7 @@ int read_meshletdata(NvcContext* ctx, cudaStream_t stream, const void* file, siz
 	if (e == cudaSuccess)
 		e = cudaMemcpy(&corrupt, a.corrupt, 4, cudaMemcpyDeviceToHost);
 	if (e != cudaSuccess)
-		return cuda_fail(ctx, e);
+		return nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 	return corrupt ? NVC_ERROR_CORRUPT : NVC_OK;
 }
 
@@ -135,28 +112,22 @@ extern "C" NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream
 	const NvcSceneCacheSection& sec = info->sections[section];
 	if (dst_bytes < sec.decoded_bytes || sec.offset > file_size || sec.stored_bytes > file_size - sec.offset)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	int current = -1;
-	if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
-	{
-		ctx->last_error = "the context's CUDA device is not the calling thread's current device";
+	if (!nvc::device_is_current(ctx))
 		return NVC_ERROR_INVALID_ARGUMENT;
-	}
 	const uint8_t* data = static_cast<const uint8_t*>(file) + sec.offset;
 	const cudaStream_t s = static_cast<cudaStream_t>(stream);
-	// the caller's earlier work on `stream` and the previous call's use of the scratch finish before the copies below,
-	// which are not ordered with `stream` (see upload)
+	// the caller's earlier work on `stream` and the previous user of the scratch finish before the copies below, which are not
+	// ordered with `stream` (nvc::upload)
 	cudaError_t e = cudaDeviceSynchronize();
 	if (e != cudaSuccess)
-		return cuda_fail(ctx, e);
+		return nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 
 	if (!sec.compressed)
 	{
 		if (sec.decoded_bytes > sec.stored_bytes)
 			return NVC_ERROR_INVALID_ARGUMENT;
-		e = upload(dst, data, sec.decoded_bytes);
-		if (e == cudaSuccess)
-			e = cudaDeviceSynchronize();
-		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e);
+		e = nvc::upload({ { dst, data, sec.decoded_bytes } });
+		return e == cudaSuccess ? NVC_OK : nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 	}
 	// the kernels and their index address the staged stream with 32-bit offsets
 	if (section != NVC_CACHE_INDICES && sec.stored_bytes > 0xffffffffull)
@@ -171,10 +142,8 @@ extern "C" NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream
 		int status = nvc::decode_index_stream(data, sec.stored_bytes, sec.count, indices.data());
 		if (status != NVC_OK)
 			return status;
-		e = upload(dst, indices.data(), sec.decoded_bytes);
-		if (e == cudaSuccess)
-			e = cudaDeviceSynchronize();
-		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e);
+		e = nvc::upload({ { dst, indices.data(), sec.decoded_bytes } });
+		return e == cudaSuccess ? NVC_OK : nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 	}
 	if (section != NVC_CACHE_MESHLETDATA)
 		return NVC_ERROR_UNSUPPORTED;

@@ -22,12 +22,6 @@ struct Encoded
 	uint64_t bytes = 0;
 };
 
-int cuda_fail(NvcContext* ctx, cudaError_t e)
-{
-	ctx->last_error = std::string("nvc_scene_cache_write: ") + cudaGetErrorString(e);
-	return e == cudaErrorMemoryAllocation ? NVC_ERROR_OUT_OF_MEMORY : NVC_ERROR_CUDA;
-}
-
 bool on_device(const NvcSceneCacheWriteDesc* d, int s)
 {
 	return (d->device_sections >> s) & 1u;
@@ -133,16 +127,12 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 		uses_device = uses_device || on_device(d, s) || device_encoded(d, s);
 	if (uses_device)
 	{
-		int current = -1;
-		if (cudaGetDevice(&current) != cudaSuccess || current != ctx->device)
-		{
-			ctx->last_error = "the context's CUDA device is not the calling thread's current device";
+		if (!nvc::device_is_current(ctx))
 			return NVC_ERROR_INVALID_ARGUMENT;
-		}
 		// the caller's work on `stream` (which produced the device arrays) and the previous user of the scratch finish first
 		cudaError_t e = cudaDeviceSynchronize();
 		if (e != cudaSuccess)
-			return cuda_fail(ctx, e);
+			return nvc::load_fail(ctx, e, "nvc_scene_cache_write");
 	}
 	const cudaStream_t cs = static_cast<cudaStream_t>(stream);
 	Encoded enc[NVC_CACHE_SECTION_COUNT];
@@ -196,12 +186,12 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 		char* base = nullptr;
 		if (plan.bytes)
 		{
-			e = nvc::reserve_cache_scratch(ctx, plan.bytes);
-			base = static_cast<char*>(ctx->cache_scratch);
-			for (int s = 0; s < NVC_CACHE_SECTION_COUNT && e == cudaSuccess; ++s)
-				if (staged[s] && raw_bytes(d, s))
-					e = cudaMemcpy(base + in_at[s], d->data[s], raw_bytes(d, s), cudaMemcpyHostToDevice);
+			e = nvc::reserve_scratch(ctx, plan.bytes);
+			base = static_cast<char*>(ctx->load_scratch);
 		}
+		auto input = [&](int s) { return nvc::Upload{ base + in_at[s], d->data[s], staged[s] ? size_t(raw_bytes(d, s)) : 0 }; };
+		if (e == cudaSuccess && uses_device)
+			e = nvc::upload({ input(NVC_CACHE_VERTICES), input(NVC_CACHE_MESHLETVTX0), input(NVC_CACHE_MESHLETS), input(NVC_CACHE_MESHLETDATA) });
 		// indices in device memory come down before the kernels are queued, so that the copy does not wait for them
 		std::vector<uint32_t> indices;
 		const uint32_t* index_src = static_cast<const uint32_t*>(d->data[NVC_CACHE_INDICES]);
@@ -211,9 +201,6 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 			e = cudaMemcpy(indices.data(), index_src, indices.size() * 4, cudaMemcpyDeviceToHost);
 			index_src = indices.data();
 		}
-		// the uploads from pageable memory are not ordered with a non-blocking `stream`
-		if (e == cudaSuccess && uses_device)
-			e = cudaDeviceSynchronize();
 		for (int i = 0; i < 2 && e == cudaSuccess; ++i)
 		{
 			const int s = int(vertex_sections[i]);
@@ -237,7 +224,7 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 			e = nvc::launch_encode_meshlets(ma, cs);
 		}
 		if (e != cudaSuccess)
-			return cuda_fail(ctx, e);
+			return nvc::load_fail(ctx, e, "nvc_scene_cache_write");
 
 		// the index stream, on the host while the kernels run
 		index_stream.reset(new uint8_t[nvc::index_stream_bound(d->count[NVC_CACHE_INDICES])]);
@@ -263,7 +250,7 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 			enc[NVC_CACHE_MESHLETDATA].bytes = section_bytes;
 		}
 		if (e != cudaSuccess)
-			return cuda_fail(ctx, e);
+			return nvc::load_fail(ctx, e, "nvc_scene_cache_write");
 		if (invalid)
 		{
 			ctx->last_error = "nvc_scene_cache_write: a meshlet's words lie outside meshletdata, or it has more than 64 vertices or 96 triangles";
@@ -313,7 +300,7 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 	memcpy(out, &h, sizeof(h));
 	size_t at = sizeof(h);
 	cudaError_t e = cudaSuccess;
-	const char* base = static_cast<const char*>(ctx ? ctx->cache_scratch : nullptr);
+	const char* base = static_cast<const char*>(ctx ? ctx->load_scratch : nullptr);
 	for (int s = 0; s < NVC_CACHE_SECTION_COUNT && e == cudaSuccess; ++s)
 	{
 		const bool coded = d->compressed && (s == NVC_CACHE_VERTICES || s == NVC_CACHE_INDICES || s == NVC_CACHE_MESHLETDATA || s == NVC_CACHE_MESHLETVTX0);
@@ -347,7 +334,7 @@ extern "C" NVC_API int nvc_scene_cache_write(NvcContext* ctx, void* stream, cons
 		at += n;
 	}
 	if (e != cudaSuccess)
-		return cuda_fail(ctx, e);
+		return nvc::load_fail(ctx, e, "nvc_scene_cache_write");
 	*file_size = at;
 	return NVC_OK;
 }

@@ -1,6 +1,5 @@
-// TEST INFRASTRUCTURE — guarded device allocations for the emulated library (tests/test_meshlet_view.py).  Linked into a
-// separate build of the emulation with -Wl,--wrap=calloc,--wrap=free, so that the emulated cudaMalloc / cudaFree
-// (calloc / free) of that build come here.  While emu_guard_allocations(1) is in effect, every allocation is placed so
+// TEST INFRASTRUCTURE — guarded device allocations for the emulated library (tests/emu_lib.py).  Linked into it with
+// -Wl,--wrap=calloc,--wrap=free, so that the emulated cudaMalloc / cudaFree (calloc / free) come here.  While emu_guard_allocations(1) is in effect, every allocation is placed so
 // that it ends exactly at an inaccessible page: a kernel that reads past the end of a context-owned buffer faults, the
 // CPU counterpart of compute-sanitizer's memcheck.  Otherwise the calls go to the C library unchanged.
 #include <stddef.h>

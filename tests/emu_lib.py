@@ -22,24 +22,32 @@ _LIB = None
 
 
 def load():
-    """Builds (when stale) and loads the emulated library."""
+    """Builds (when stale) and loads the emulated library: the translated kernels and API, the emulation, the host sources
+    (nvc_host, the scene-cache reader and writer and their codecs) and cuda_emu/guard_alloc.cpp.  Its calloc / free are
+    wrapped: after emu_guard_allocations(1) every device allocation ends exactly at an inaccessible page, so that a kernel
+    that reads past a context-owned buffer faults; until then every call goes to the C library."""
     global _LIB
     so = os.path.join(OUT, "libniagara_cull_emu.so")
     if _LIB is not None:
         return _LIB
     os.makedirs(OUT, exist_ok=True)
-    srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(EMU, f) for f in ("gen_emu.py", "emu.cpp", "emu_stubs.cpp")] + [os.path.join(EMU, "include", f) for f in os.listdir(os.path.join(EMU, "include"))] + [os.path.join(ROOT, "include", "niagara_cull.h")]
+    emu = [os.path.join(EMU, f) for f in ("emu.cpp", "emu_stubs.cpp", "guard_alloc.cpp")]
+    host = [os.path.join(CSRC, f + ".cpp") for f in ("nvc_host", "nvc_scene_cache", "nvc_scene_cache_device", "nvc_scene_cache_write", "nvc_meshopt_decode", "nvc_meshopt_encode")]
+    srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + emu + [os.path.join(EMU, "gen_emu.py")] + [os.path.join(EMU, "include", f) for f in os.listdir(os.path.join(EMU, "include"))] + [os.path.join(ROOT, "include", "niagara_cull.h")]
     if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         for name in ("nvc_kernels", "nvc_api"):
             subprocess.run(["python3", os.path.join(EMU, "gen_emu.py"), os.path.join(CSRC, name + ".cu"), os.path.join(OUT, name + ".cpp")], check=True)
         cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I", os.path.join(EMU, "include"), "-I", CSRC]
-        cmd += ["-o", so, os.path.join(OUT, "nvc_kernels.cpp"), os.path.join(OUT, "nvc_api.cpp"), os.path.join(EMU, "emu.cpp"), os.path.join(EMU, "emu_stubs.cpp"), os.path.join(CSRC, "nvc_host.cpp")]
+        cmd += ["-Wl,--wrap=calloc,--wrap=free", "-o", so, os.path.join(OUT, "nvc_kernels.cpp"), os.path.join(OUT, "nvc_api.cpp")] + emu + host
         subprocess.run(cmd, check=True)
     lib = ctypes.CDLL(so)
     for name, restype, argtypes in product_lib.SIGNATURES:
         if hasattr(lib, name):
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = restype, argtypes
+    lib.emu_guard_allocations.argtypes = [ctypes.c_int]
+    lib.emu_guard_allocations.restype = None
+    lib.emu_guarded_live.restype = ctypes.c_int
     _LIB = lib
     return lib
 

@@ -286,17 +286,17 @@ def test_restatement_matches_fixtures(name):
     assert wm.tobytes() == meshes.tobytes() and np.array_equal(wib, ib), name
 
 
-def end_to_end_emulated(ref_file, raw, clrt):
-    """nvc_cook_mesh_lods -> nvc_cook_meshlets(_clrt) -> nvc_scene_cache_write, all emulated, from the run's Vertex[] and LOD 0"""
+def end_to_end_emulated(emu, ref_file, raw, clrt):
+    """nvc_cook_mesh_lods -> nvc_cook_meshlets(_clrt) -> nvc_scene_cache_write, all emulated on one context, from the run's
+    Vertex[] and LOD 0"""
     import test_scene_cache_write as write_tests
 
-    lib, ctx = write_tests.emu()
+    lib, ctx = emu.lib, emu.ctx
     header, secs = raw_geometry(raw)
     header.clrtMode = int(clrt)
     v = secs["vertices"].view(np.uint16).reshape(-1, 8)
     stored = secs["meshes"].view(layout.MESH_DTYPE)
     scale = max_scale_of("animated_clrt" if clrt else raw, len(stored))
-    # lods: the emulated library that also holds the writer
     cap = capacity(lib, lod0_input(stored))
     meshes = np.zeros(len(stored), layout.MESH_DTYPE)
     ib = np.zeros(cap + 1, np.uint32)
@@ -334,10 +334,10 @@ def end_to_end_emulated(ref_file, raw, clrt):
 
 
 @pytest.mark.parametrize("ref_file,raw,clrt", END_TO_END)
-def test_end_to_end_emulated(ref_file, raw, clrt):
+def test_end_to_end_emulated(emu, ref_file, raw, clrt):
     """Vertex[] and LOD 0 -> LOD chains -> meshlets -> compressed cache: the reference's file, byte for byte"""
     want = np.fromfile(os.path.join(GOLDEN, ref_file), np.uint8)
-    got = end_to_end_emulated(ref_file, raw, clrt)
+    got = end_to_end_emulated(emu, ref_file, raw, clrt)
     assert len(got) == len(want) and np.array_equal(got, want), ref_file
 
 
@@ -530,12 +530,11 @@ def test_capacity_and_overflow(emu):
 
 
 def test_rejected_mesh_reads_no_vertex():
-    """a rejected mesh's vertices lie past the end of an array that ends at an inaccessible page, in the build whose device
+    """a rejected mesh's vertices lie past the end of an array that ends at an inaccessible page, and the call's device
     allocations end at one too: reading any of them, or past any scratch array, faults"""
     import test_scene_cache_device as dev_tests
-    import test_scene_cache_write as write_tests
 
-    lib, _ = write_tests.emu(guard=True)
+    lib = emu_lib.load()
     rng = np.random.default_rng(13)
     p, n, i = grid_mesh(rng, 4, 4)
     good = make_vertices(p, n)

@@ -6,7 +6,7 @@ meshlet.mesh.glsl with `#define CULL 1` (oracle/_ref/librefshader_cull.so), and 
 the shader flags gl_CullPrimitiveEXT.
 CPU tier: the product's kernels under the SIMT emulation (tests/cuda_emu) against that shader + the test rasteriser, bit for bit:
 whole frames in both modes, single decisions on constructed triangles, closed two-phase loops against the brute-force image, the
-switch turned off again, and hostile meshlet data in the guarded-memory build.
+switch turned off again, and hostile meshlet data in guarded memory.
 GPU tier (-m gpu): the same loops and a 2 000-draw frame per mode on the device."""
 import ctypes
 import os
@@ -20,7 +20,6 @@ import refshader_lib
 from niagara_b200 import host, layout, scenes
 from test_end_to_end_raster import _all_clusters, _kitten_scene
 from test_kernels_emulated import _guarded
-from test_meshlet_view import _guard_alloc_library
 from test_raster_submission_modes import _EmuPath as _ModesEmuPath
 from test_raster_submission_modes import _bits, _cache_geometry, _payloads_from_cib, _task_buffers
 
@@ -508,7 +507,7 @@ def test_switching_off_restores_the_default_producer(golden_dir):
 
 def test_hostile_meshlets_with_mesh_cull_in_guarded_memory(golden_dir):
     """out-of-range meshlet data, vertex references and triangle indices with the stage on: the same rejections, stats4[2] and image as
-    with it off, in the build whose every input array ends at an inaccessible page (any read past an end faults)"""
+    with it off, with every input array ending at an inaccessible page (any read past an end faults)"""
     screen = (128, 96)
     s, vertices, meshletdata = _kitten_scene(golden_dir, 40, screen)
     cd = s.cull_data(culling=False, occlusion=False, cluster_occlusion=False)
@@ -523,7 +522,7 @@ def test_hostile_meshlets_with_mesh_cull_in_guarded_memory(golden_dir):
     count = int(o.ccb[0])
     cib_live = o.cib[:count].copy()
     payloads, emit = _payloads_from_cib(o.cib, count, ncmd)
-    lib = _guard_alloc_library()
+    lib = emu_lib.load()
     ctx = ctypes.c_void_p()
     lib.emu_guard_allocations(1)  # the context's device allocations (the counters among them) end at a guard page too
     try:

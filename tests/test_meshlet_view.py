@@ -4,7 +4,6 @@ oracle's results bit for bit, in the filtered and the exact kernel, for cluster-
 whose Meshlet[] pointer is not the prepared one must read the records."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -12,7 +11,6 @@ import pytest
 import emu_lib
 import oracle_lib
 from niagara_b200 import layout, scenes
-from niagara_b200 import lib as product_lib
 from test_kernels_emulated import _compare_clusters, _compare_draw, _guarded
 
 
@@ -40,28 +38,6 @@ def _paths(s, view, **kw):
     o.set_visibility_bits(s.visibility_bits)
     e.set_visibility_bits(s.visibility_bits)
     return o, e
-
-
-def _guard_alloc_library():
-    """The emulated library once more, linked with tests/cuda_emu/guard_alloc.cpp so that its cudaMalloc can place allocations
-    against an inaccessible page (emu_guard_allocations)."""
-    emu_lib.load()  # (re)generates the translated kernel sources of the current tree
-    so = os.path.join(emu_lib.OUT, "libniagara_cull_emu_guard_alloc.so")
-    guard = os.path.join(emu_lib.EMU, "guard_alloc.cpp")
-    objs = [os.path.join(emu_lib.OUT, "nvc_kernels.cpp"), os.path.join(emu_lib.OUT, "nvc_api.cpp"), os.path.join(emu_lib.EMU, "emu.cpp"), os.path.join(emu_lib.EMU, "emu_stubs.cpp"), os.path.join(emu_lib.CSRC, "nvc_host.cpp"), guard]
-    if not os.path.exists(so) or any(os.path.getmtime(f) > os.path.getmtime(so) for f in objs):
-        cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I", os.path.join(emu_lib.EMU, "include"), "-I", emu_lib.CSRC]
-        cmd += ["-Wl,--wrap=calloc,--wrap=free", "-o", so] + objs
-        subprocess.run(cmd, check=True)
-    lib = ctypes.CDLL(so)
-    for name, restype, argtypes in product_lib.SIGNATURES:
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = restype, argtypes
-    lib.emu_guard_allocations.argtypes = [ctypes.c_int]
-    lib.emu_guard_allocations.restype = None
-    lib.emu_guarded_live.restype = ctypes.c_int
-    return lib
 
 
 def _task_table(p, n, payloads, counts):
@@ -174,8 +150,7 @@ def test_view_arrays_end_at_guard_page(golden_dir):
     past either array's end would fault."""
     s = _kitten(golden_dir, 2047)
     o, e = _paths(s, False)
-    e.close()  # the same buffers, driven by the build whose allocations can be guarded
-    e.emu = _guard_alloc_library()
+    e.close()  # the same buffers, driven through a fresh context
     e.ctx = ctypes.c_void_p()
     limits = layout.Limits(e.limits.task_wglimit, e.limits.cluster_limit)
     assert e.emu.nvc_create(0, ctypes.byref(limits), ctypes.byref(e.ctx)) == 0

@@ -1,19 +1,17 @@
 """nvc_scene_cache_read_device: every section of a scene cache read into device memory equals nvc_scene_cache_read's bytes and
-status.  The CPU tier runs the product's kernels under the SIMT emulation, in a build of the emulated library that also links
-the scene-cache sources (plain, and with allocations that end at an inaccessible page); the GPU tier reads the same caches
+status.  The CPU tier runs the product's kernels under the SIMT emulation (tests/emu_lib.py), some reads with allocations that
+end at an inaccessible page; the GPU tier reads the same caches
 through SceneCache.section_device.  Synthetic caches are built here from streams of the reference's encoders
 (oracle/_ref/libmeshopt_ref.so) and skip where that library was not built."""
 import ctypes
 import mmap
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import emu_lib
 from niagara_b200 import layout
-from niagara_b200 import lib as product_lib
 from niagara_b200.lib import load_library
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -28,36 +26,17 @@ vp, sz = ctypes.c_void_p, ctypes.c_size_t
 needs_ref = pytest.mark.skipif(not os.path.exists(REF_SO), reason="needs the reference's codecs (oracle/_ref/libmeshopt_ref.so)")
 
 
-# ---- the emulated library with the scene-cache sources -------------------------------------------------------------------
-_EMU = {}
+# ---- the emulated library and a context of it -----------------------------------------------------------------------------
+_CTX = []
 
 
-def _emu(guard=False):
-    if guard in _EMU:
-        return _EMU[guard]
-    emu_lib.load()  # (re)generates the translated kernel sources of the current tree
-    so = os.path.join(emu_lib.OUT, "libniagara_cull_emu_cache%s.so" % ("_guard" if guard else ""))
-    srcs = [os.path.join(emu_lib.OUT, "nvc_kernels.cpp"), os.path.join(emu_lib.OUT, "nvc_api.cpp"), os.path.join(emu_lib.EMU, "emu.cpp"), os.path.join(emu_lib.EMU, "emu_stubs.cpp")]
-    srcs += [os.path.join(emu_lib.CSRC, f) for f in ("nvc_host.cpp", "nvc_scene_cache.cpp", "nvc_scene_cache_device.cpp", "nvc_meshopt_decode.cpp")]
-    srcs += [os.path.join(emu_lib.EMU, "guard_alloc.cpp")] if guard else []
-    deps = srcs + [os.path.join(emu_lib.CSRC, f) for f in os.listdir(emu_lib.CSRC)]
-    if not os.path.exists(so) or any(os.path.getmtime(f) > os.path.getmtime(so) for f in deps):
-        cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I", os.path.join(emu_lib.EMU, "include"), "-I", emu_lib.CSRC]
-        cmd += (["-Wl,--wrap=calloc,--wrap=free"] if guard else []) + ["-o", so] + srcs
-        subprocess.run(cmd, check=True)
-    lib = ctypes.CDLL(so)
-    for name, restype, argtypes in product_lib.SIGNATURES:
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = restype, argtypes
-    if guard:
-        lib.emu_guard_allocations.argtypes = [ctypes.c_int]
-        lib.emu_guard_allocations.restype = None
-        lib.emu_guarded_live.restype = ctypes.c_int
-    ctx = ctypes.c_void_p()
-    assert lib.nvc_create(0, None, ctypes.byref(ctx)) == 0
-    _EMU[guard] = (lib, ctx)
-    return lib, ctx
+def _emu():
+    lib = emu_lib.load()
+    if not _CTX:
+        ctx = ctypes.c_void_p()
+        assert lib.nvc_create(0, None, ctypes.byref(ctx)) == 0
+        _CTX.append(ctx)
+    return lib, _CTX[0]
 
 
 _KEEP = []
@@ -91,7 +70,7 @@ def _host_read(data, info, s):
 def _device_read(data, info, s, guard=False, fill=0xEE):
     """Guarded: a fresh context, so that its scratch is allocated for this read alone and ends where the staged stream's
     last word does, against an inaccessible page, as `dst` does; a read or write past either faults."""
-    lib, ctx = _emu(guard)
+    lib, ctx = _emu()
     n = int(info.sections[s].decoded_bytes)
     out = _guarded_zeros(n) if guard else np.zeros(n, np.uint8)
     out[:] = fill

@@ -1,6 +1,5 @@
 """nvc_scene_cache_write: the file saveSceneCache writes, byte for byte.  The CPU tier runs the product's encoder kernels under
-the SIMT emulation, in a build of the emulated library that also links the scene-cache sources (plain, and with allocations
-that end at an inaccessible page); the GPU tier writes through scene_cache.write_scene_cache.  The reference files are
+the SIMT emulation (tests/emu_lib.py), some writes with allocations that end at an inaccessible page; the GPU tier writes through scene_cache.write_scene_cache.  The reference files are
 tests/golden/*.z.cache with the raw geometry of the same runs (scene_cache_write_raw.npz, animated.raw.cache); the codec
 streams are compared against the reference's own encoders (oracle/_ref/libmeshopt_ref.so), skipped where that library was not
 built."""
@@ -73,41 +72,9 @@ def write(lib, ctx, desc, capacity=None, fill=0xEE):
 
 
 # ---- CPU tier ---------------------------------------------------------------------------------------------------------
-_EMU = {}
-
-
-def emu(guard=False):
-    """the emulated library with the scene-cache reader and writer (test_scene_cache_device's build plus the writer)"""
-    if guard in _EMU:
-        return _EMU[guard]
-    import subprocess
-
-    import emu_lib
-    from niagara_b200 import lib as product_lib
-
-    emu_lib.load()
-    so = os.path.join(emu_lib.OUT, "libniagara_cull_emu_write%s.so" % ("_guard" if guard else ""))
-    srcs = [os.path.join(emu_lib.OUT, "nvc_kernels.cpp"), os.path.join(emu_lib.OUT, "nvc_api.cpp"), os.path.join(emu_lib.EMU, "emu.cpp"), os.path.join(emu_lib.EMU, "emu_stubs.cpp")]
-    srcs += [os.path.join(emu_lib.CSRC, f) for f in ("nvc_host.cpp", "nvc_scene_cache.cpp", "nvc_scene_cache_device.cpp", "nvc_scene_cache_write.cpp", "nvc_meshopt_decode.cpp", "nvc_meshopt_encode.cpp")]
-    srcs += [os.path.join(emu_lib.EMU, "guard_alloc.cpp")] if guard else []
-    deps = srcs + [os.path.join(emu_lib.CSRC, f) for f in os.listdir(emu_lib.CSRC)]
-    if not os.path.exists(so) or any(os.path.getmtime(f) > os.path.getmtime(so) for f in deps):
-        cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-w", "-I", os.path.join(emu_lib.EMU, "include"), "-I", emu_lib.CSRC]
-        cmd += (["-Wl,--wrap=calloc,--wrap=free"] if guard else []) + ["-o", so] + srcs
-        subprocess.run(cmd, check=True)
-    lib = ctypes.CDLL(so)
-    for name, restype, argtypes in product_lib.SIGNATURES:
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = restype, argtypes
-    if guard:
-        lib.emu_guard_allocations.argtypes = [ctypes.c_int]
-        lib.emu_guard_allocations.restype = None
-        lib.emu_guarded_live.restype = ctypes.c_int
-    ctx = ctypes.c_void_p()
-    assert lib.nvc_create(0, None, ctypes.byref(ctx)) == 0
-    _EMU[guard] = (lib, ctx)
-    return lib, ctx
+def emu():
+    """the emulated library and a context of it (test_scene_cache_device's)"""
+    return dev_tests._emu()
 
 
 def ref_lib():
@@ -373,7 +340,7 @@ def _guarded(a):
 
 
 def test_rejections_leave_the_output_untouched():
-    lib, ctx = emu(guard=True)
+    lib, ctx = emu()
     header, secs = raw_sections(raw_file("kitten"))
     md = secs["meshletdata"].view(np.uint32)
     m = secs["meshlets"].view(layout.MESHLET_DTYPE).copy()

@@ -21,7 +21,6 @@ from niagara_b200 import host, layout
 from test_end_to_end_raster import _all_clusters, _kitten_scene
 from test_kernels_emulated import _guarded
 from test_mesh_cull import MOVING
-from test_meshlet_view import _guard_alloc_library
 from test_raster_submission_modes import _EmuPath as _ModesEmuPath
 from test_raster_submission_modes import _bits, _task_buffers
 
@@ -375,12 +374,12 @@ def _no_access(nbytes):
 
 
 def test_pass_through_in_guarded_memory(golden_dir):
-    """the guarded-memory build: outputs sized exactly and ending at an inaccessible page, draws, meshlets and mvb inaccessible as a
+    """in guarded memory: outputs sized exactly and ending at an inaccessible page, draws, meshlets and mvb inaccessible as a
     whole (the passes must not read them), the context's own allocations guarded too"""
     screen = (64, 64)
     s, _, _ = _scene(golden_dir, 4, screen)
     cd = s.cull_data(cluster_occlusion=False)
-    lib = _guard_alloc_library()
+    lib = emu_lib.load()
     ctx = ctypes.c_void_p()
     lib.emu_guard_allocations(1)
     try:
