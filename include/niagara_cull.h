@@ -457,14 +457,16 @@ typedef struct NvcSceneCacheInfo
 } NvcSceneCacheInfo;
 
 /* nvc_scene_cache_read into DEVICE memory: dst is a device pointer, 4-byte aligned, with room for
- * info->sections[section].decoded_bytes.  Raw sections are copied up.  VERTICES, MESHLETVTX0 (vertex codec) and MESHLETDATA
- * (meshlet codec) go up compressed, with an index the host finds by walking their sizes, and are decoded by kernels.
- * INDICES is decoded on the host by nvc_scene_cache_read's decoder and copied up (the index codec is one sequential FIFO
- * state machine).  Result byte for byte and status equal to nvc_scene_cache_read + a copy, except that a cache whose
+ * info->sections[section].decoded_bytes.  Raw sections are copied up.  VERTICES, MESHLETVTX0 (vertex codec), INDICES (index
+ * codec) and MESHLETDATA (meshlet codec) go up compressed, with an index the host finds by walking their sizes, and are
+ * decoded by kernels; no host copy of the decoded section is made.  INDICES is cut into chunks of 256 triangles: each
+ * chunk's effect on the decoder's FIFO state is found on its own, the effects are combined by a scan, and every chunk is
+ * then decoded from its exact entry state.  Result byte for byte and status equal to nvc_scene_cache_read + a copy, except that a cache whose
  * meshlet word ranges are not in increasing, non-overlapping order is refused with NVC_ERROR_UNSUPPORTED before anything
  * is written (every cache the reference writes is in that order: appendMeshlet appends), and a compressed VERTICES,
  * MESHLETVTX0 or MESHLETDATA stream of 4 GiB or more is refused likewise (its index holds 32-bit offsets).  On NVC_ERROR_CORRUPT the
- * contents of dst are unspecified, as on the host.  A corrupt vertex stream is found by the host walk, before any launch.
+ * contents of dst are unspecified, as on the host.  A corrupt vertex or index stream is found by the host walk, before any
+ * launch, and dst is not written.
  * Runs on `stream` and synchronises the device (it reads back a corruption flag), so it belongs at load time, outside
  * stream capture.  The staged stream and its index live in scratch the context owns, grown as needed. */
 NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream, const void* file, size_t file_size, const NvcSceneCacheInfo* info, int section,

@@ -307,5 +307,276 @@ __global__ void __launch_bounds__(kMeshletWarps * 32) decode_meshlets_kernel(con
 		atomicOr(a.corrupt, 1u);
 }
 
+// Index codec (INDICES).  The decoder's state is small: a 16-slot vertex ring, two 16-slot edge rings pushed together,
+// `next` and `last`.  A chunk of kIndexChunk triangles changes it by a substitution that does not depend on the entry
+// state: each exit slot, and the exit `next` and `last`, is a constant, entry next + k, entry last + k, or one named entry
+// slot (icodec::decode_triangle copies values between slots and only ever adds to `next` and `last`), and each ring's
+// head advances by a count the codes fix.  Substitutions compose associatively, so:
+//   symbolic  one thread per chunk runs the decoder's step from a symbolic entry state (slot j holds "entry slot j",
+//             next "entry next + 0", ...) and stores the chunk's substitution.  The host walk (walk_index_stream) has
+//             found where each chunk's data bytes start and checked the whole stream, so nothing here can fail.
+//   scan      an exclusive scan of the substitutions from the decoder's initial state (every slot 0xffffffff, next = last
+//             = 0), in three launches: one warp per run of kIndexRun chunks composes their total; one warp scans the run
+//             totals; one warp per run scans its chunks from the run's entry state.  A warp holds a substitution as
+//             kIndexEntries words over its lanes and composes with shuffles.  The result is each chunk's entry state.
+//   concrete  one thread per chunk decodes it again from its true entry state; a warp stages kIndexBatch triangles per
+//             lane in shared memory and stores each lane's run of indices as one coalesced span.
+// Rings are kept as the host decoder keeps them, physical slots and a head, including the slot a FIFO hit writes without
+// advancing; a substitution's slots are named relative to the heads at its entry.  The exact serial decoder's state is
+// reproduced at every chunk's entry.  Symbolic values are uint2 { tag, k }: tag < 48 names an entry slot (vertex ring 0 ..
+// 15, edge ring a 16 .. 31, edge ring b 32 .. 47), kTagNext / kTagLast entry next / last + k, kTagConst the constant k.
+// Word kIndexEntries - 1 of a substitution holds its head advances { vertex, edge }.
+constexpr uint32_t kIndexThreads = 64;
+constexpr uint32_t kIndexBatch = 8;                         // triangles a lane stages between coalesced stores
+constexpr uint32_t kIndexStageStride = kIndexBatch * 3 + 1; // words per lane, odd: the lanes' staging stores miss each other's banks
+constexpr uint32_t kIndexScanWarps = 4;
+constexpr uint32_t kTagNext = 48, kTagLast = 49, kTagConst = 50;
+
+__device__ __forceinline__ uint32_t index_add(uint32_t v, uint32_t k)
+{
+	return v + k;
+}
+
+__device__ __forceinline__ uint2 index_add(uint2 v, uint32_t k)
+{
+	return make_uint2(v.x, v.y + k);
+}
+
+// The decoder's state for icodec::decode_triangle with its rings in shared memory: slot j of this thread's 48 at
+// ring[j * kIndexThreads] (the threads of a warp always touch distinct banks)
+template <typename V>
+struct SharedIndexState
+{
+	using Value = V;
+	V* ring;
+	uint32_t vhead, ehead;
+	V next, last;
+	__device__ __forceinline__ static V add(V v, uint32_t k) { return index_add(v, k); }
+	__device__ __forceinline__ static V zero() { return index_add(V(), 0u) ; }
+	__device__ __forceinline__ V vert(uint32_t n) const { return ring[((vhead - n) & 15u) * kIndexThreads]; }
+	__device__ __forceinline__ V edge_a(uint32_t n) const { return ring[(16u + ((ehead - n) & 15u)) * kIndexThreads]; }
+	__device__ __forceinline__ V edge_b(uint32_t n) const { return ring[(32u + ((ehead - n) & 15u)) * kIndexThreads]; }
+	__device__ __forceinline__ void put_vert(V v, bool advance)
+	{
+		ring[vhead * kIndexThreads] = v;
+		vhead = (vhead + (advance ? 1u : 0u)) & 15u;
+	}
+	__device__ __forceinline__ void put_edge(V a, V b)
+	{
+		ring[(16u + ehead) * kIndexThreads] = a;
+		ring[(32u + ehead) * kIndexThreads] = b;
+		ehead = (ehead + 1u) & 15u;
+	}
+};
+
+template <>
+__device__ __forceinline__ uint2 SharedIndexState<uint2>::zero()
+{
+	return make_uint2(kTagConst, 0u);
+}
+
+// a chunk's data bytes, where the host walk found them
+struct IndexBytes
+{
+	const uint8_t* at;
+	__device__ __forceinline__ bool next(uint32_t& b)
+	{
+		b = __ldg(at++);
+		return true;
+	}
+};
+
+// the 16-byte aux table into shared memory, before any thread returns
+__device__ __forceinline__ void load_index_aux(const IndexDecodeArgs& a, uint8_t* s_aux)
+{
+	if (threadIdx.x < 16)
+		s_aux[threadIdx.x] = __ldg(a.stream + a.aux_offset + threadIdx.x);
+	__syncthreads();
+}
+
+template <typename V>
+// triangles first .. first + count - 1 of chunk c; stage (when not null) receives their corners from stage[0] on
+__device__ __forceinline__ void decode_index_chunk(SharedIndexState<V>& s, const IndexDecodeArgs& a, const uint8_t* aux, uint32_t c, uint32_t first, uint32_t count,
+    IndexBytes& data, V* stage)
+{
+	for (uint32_t t = first; t < first + count; ++t)
+	{
+		V corner[3];
+		icodec::decode_triangle(s, __ldg(a.stream + 1 + size_t(c) * kIndexChunk + t), aux, a.direct_slots, data, corner);
+		if (stage)
+			for (uint32_t j = 0; j < 3; ++j)
+				stage[(t - first) * 3 + j] = corner[j];
+	}
+}
+
+__global__ void __launch_bounds__(kIndexThreads) decode_index_symbolic_kernel(const IndexDecodeArgs a)
+{
+	__shared__ uint2 s_ring[48 * kIndexThreads];
+	__shared__ uint8_t s_aux[16];
+	load_index_aux(a, s_aux);
+	const uint32_t c = blockIdx.x * kIndexThreads + threadIdx.x;
+	if (c >= a.chunks)
+		return;
+	SharedIndexState<uint2> s = { s_ring + threadIdx.x, 0u, 0u, make_uint2(kTagNext, 0u), make_uint2(kTagLast, 0u) };
+	for (uint32_t j = 0; j < 48; ++j)
+		s.ring[j * kIndexThreads] = make_uint2(j, 0u);
+	IndexBytes data = { a.stream + a.chunk_data[c] };
+	decode_index_chunk<uint2>(s, a, s_aux, c, 0, min(kIndexChunk, a.triangles - c * kIndexChunk), data, nullptr);
+	for (uint32_t j = 0; j < 48; ++j)
+		a.sub[size_t(j) * a.chunks + c] = s.ring[j * kIndexThreads];
+	a.sub[size_t(48) * a.chunks + c] = s.next;
+	a.sub[size_t(49) * a.chunks + c] = s.last;
+	a.sub[size_t(50) * a.chunks + c] = make_uint2(s.vhead, s.ehead);
+}
+
+__device__ __forceinline__ uint2 shfl2(uint2 v, uint32_t src)
+{
+	return make_uint2(__shfl_sync(0xffffffffu, v.x, src), __shfl_sync(0xffffffffu, v.y, src));
+}
+
+// A substitution held by a warp: entry `lane` in lo, entry 32 + lane in hi (lanes 0 .. 17), the head advances in heads
+struct IndexSub
+{
+	uint2 lo, hi, heads;
+};
+
+__device__ __forceinline__ IndexSub load_index_sub(const uint2* buf, size_t n, size_t i)
+{
+	const uint32_t lane = threadIdx.x & 31u;
+	IndexSub s;
+	s.lo = buf[lane * n + i];
+	s.hi = lane < 18 ? buf[(32 + lane) * n + i] : make_uint2(kTagConst, 0u);
+	// lane 0 alone reads and writes the heads word, so that a warp that overwrites substitutions with entry states in
+	// place never reads a word another lane has written
+	const uint2 h = lane == 0 ? buf[size_t(kIndexEntries - 1) * n + i] : make_uint2(0u, 0u);
+	s.heads = shfl2(h, 0);
+	return s;
+}
+
+__device__ __forceinline__ void store_index_sub(uint2* buf, size_t n, size_t i, const IndexSub& s)
+{
+	const uint32_t lane = threadIdx.x & 31u;
+	buf[lane * n + i] = s.lo;
+	if (lane < 18)
+		buf[(32 + lane) * n + i] = s.hi;
+	if (lane == 0)
+		buf[size_t(kIndexEntries - 1) * n + i] = s.heads;
+}
+
+// b's value v, whose tags name slots at b's entry = a's exit, in terms of a's entry
+__device__ __forceinline__ uint2 resolve_index_value(const IndexSub& a, uint2 v)
+{
+	const uint32_t src = v.x < 16 ? (a.heads.x + v.x) & 15u : v.x < 48 ? (v.x & 48u) + ((a.heads.y + v.x) & 15u) : v.x;
+	const uint2 lo = shfl2(a.lo, src & 31u), hi = shfl2(a.hi, src & 31u);
+	const uint2 r = src < 32 ? lo : hi;
+	return v.x >= kTagConst ? v : make_uint2(r.x, r.y + v.y);
+}
+
+// a then b.  b's exit slot j is a's exit-relative slot j, the slot (j - a's advance) relative to a's entry heads
+__device__ __forceinline__ IndexSub compose_index(const IndexSub& a, const IndexSub& b)
+{
+	const uint32_t lane = threadIdx.x & 31u;
+	const uint2 lo = shfl2(b.lo, (lane & 16u) | ((lane - (lane < 16 ? a.heads.x : a.heads.y)) & 15u));
+	const uint2 hi = shfl2(b.hi, lane < 16 ? (lane - a.heads.y) & 15u : lane);
+	IndexSub r;
+	r.lo = resolve_index_value(a, lo);
+	r.hi = resolve_index_value(a, hi);
+	r.heads = make_uint2((a.heads.x + b.heads.x) & 15u, (a.heads.y + b.heads.y) & 15u);
+	return r;
+}
+
+// the substitution that changes nothing, and the decoder's initial state as one (every value constant)
+__device__ __forceinline__ IndexSub identity_index_sub()
+{
+	const uint32_t lane = threadIdx.x & 31u;
+	return { make_uint2(lane, 0u), make_uint2(32u + lane, 0u), make_uint2(0u, 0u) };
+}
+
+__device__ __forceinline__ IndexSub initial_index_state()
+{
+	const uint32_t lane = threadIdx.x & 31u;
+	return { make_uint2(kTagConst, 0xffffffffu), make_uint2(kTagConst, lane < 16 ? 0xffffffffu : 0u), make_uint2(0u, 0u) };
+}
+
+// kPrefix false: each run's total into a.run.  kPrefix true: from each run's entry state (a.run), each chunk's entry
+// state over its substitution in a.sub.  One warp per run, the next chunk's substitution loaded while one is composed.
+template <bool kPrefix>
+__global__ void __launch_bounds__(kIndexScanWarps * 32) decode_index_scan_kernel(const IndexDecodeArgs a)
+{
+	const uint32_t r = blockIdx.x * kIndexScanWarps + (threadIdx.x >> 5);
+	if (r >= a.runs)
+		return; // whole warps
+	const uint32_t first = r * kIndexRun, end = min(first + kIndexRun, a.chunks);
+	IndexSub acc = kPrefix ? load_index_sub(a.run, a.runs, r) : identity_index_sub();
+	IndexSub b = load_index_sub(a.sub, a.chunks, first);
+	for (uint32_t c = first; c < end; ++c)
+	{
+		const IndexSub next = c + 1 < end ? load_index_sub(a.sub, a.chunks, c + 1) : b;
+		if (kPrefix)
+			store_index_sub(a.sub, a.chunks, c, acc);
+		acc = compose_index(acc, b);
+		b = next;
+	}
+	if (!kPrefix)
+		store_index_sub(a.run, a.runs, r, acc);
+}
+
+// one warp: the runs' totals in a.run become their entry states
+__global__ void __launch_bounds__(32) decode_index_runs_kernel(const IndexDecodeArgs a)
+{
+	IndexSub acc = initial_index_state();
+	IndexSub b = load_index_sub(a.run, a.runs, 0);
+	for (uint32_t r = 0; r < a.runs; ++r)
+	{
+		const IndexSub next = r + 1 < a.runs ? load_index_sub(a.run, a.runs, r + 1) : b;
+		store_index_sub(a.run, a.runs, r, acc);
+		acc = compose_index(acc, b);
+		b = next;
+	}
+}
+
+__global__ void __launch_bounds__(kIndexThreads) decode_index_concrete_kernel(const IndexDecodeArgs a)
+{
+	__shared__ uint32_t s_ring[48 * kIndexThreads];
+	__shared__ uint32_t s_stage[kIndexThreads / 32][32 * kIndexStageStride];
+	__shared__ uint8_t s_aux[16];
+	load_index_aux(a, s_aux);
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	const uint32_t warp_first = blockIdx.x * kIndexThreads + warp * 32u, c = warp_first + lane;
+	if (warp_first >= a.chunks)
+		return; // whole warps
+	const bool active = c < a.chunks;
+	const uint32_t count = active ? min(kIndexChunk, a.triangles - c * kIndexChunk) : 0u;
+	SharedIndexState<uint32_t> s = { s_ring + threadIdx.x, 0u, 0u, 0u, 0u };
+	IndexBytes data = { a.stream };
+	if (active)
+	{
+		for (uint32_t j = 0; j < 48; ++j)
+			s.ring[j * kIndexThreads] = a.sub[size_t(j) * a.chunks + c].y;
+		s.next = a.sub[size_t(48) * a.chunks + c].y;
+		s.last = a.sub[size_t(49) * a.chunks + c].y;
+		const uint2 heads = a.sub[size_t(50) * a.chunks + c];
+		s.vhead = heads.x;
+		s.ehead = heads.y;
+		data.at = a.stream + a.chunk_data[c];
+	}
+	uint32_t* stage = s_stage[warp];
+	for (uint32_t b = 0; b < kIndexChunk; b += kIndexBatch)
+	{
+		const uint32_t n = count > b ? min(kIndexBatch, count - b) : 0u;
+		decode_index_chunk<uint32_t>(s, a, s_aux, c, b, n, data, stage + lane * kIndexStageStride);
+		__syncwarp();
+		for (uint32_t l = 0; l < 32; ++l)
+		{
+			const uint32_t cl = warp_first + l;
+			const uint32_t nl = cl < a.chunks ? min(kIndexChunk, a.triangles - cl * kIndexChunk) : 0u;
+			const uint32_t words = nl > b ? min(kIndexBatch, nl - b) * 3u : 0u;
+			if (lane < words)
+				a.out[(size_t(cl) * kIndexChunk + b) * 3 + lane] = stage[l * kIndexStageStride + lane];
+		}
+		__syncwarp();
+	}
+}
+
 } // namespace cache
 } // namespace nvc

@@ -351,6 +351,20 @@ struct MeshletDecodeArgs
 	uint32_t* corrupt; // set to 1 by a malformed block
 };
 cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stream);
+constexpr uint32_t kIndexChunk = 256;   // triangles per chunk of the index decoder
+constexpr uint32_t kIndexRun = 256;     // chunks per run of its combine step
+constexpr uint32_t kIndexEntries = 51;  // uint2 words of a chunk's state substitution (nvc_cache_decode.cuh)
+struct IndexDecodeArgs
+{
+	const uint8_t* stream;      // the section as stored
+	const uint64_t* chunk_data; // [chunks]: offset of each chunk's first data byte in `stream` (walk_index_stream)
+	uint2* sub;                 // [kIndexEntries][chunks]: each chunk's substitution, then its entry state
+	uint2* run;                 // [kIndexEntries][runs]: each run's substitution, then its entry state
+	uint32_t* out;              // triangles * 3 indices
+	uint64_t aux_offset;        // of the 16-byte aux table in `stream`
+	uint32_t triangles, chunks, runs, direct_slots;
+};
+cudaError_t launch_decode_indices(const IndexDecodeArgs& a, cudaStream_t stream);
 // Sub-allocations of the context's load-time scratch, each 256-byte aligned; `bytes` ends where the last one does
 struct ScratchPlan
 {

@@ -3752,6 +3752,26 @@ cudaError_t launch_decode_meshlets(const MeshletDecodeArgs& a, cudaStream_t stre
 	return cudaGetLastError();
 }
 
+// nvc_scene_cache_read_device: the index codec's symbolic pass, three-launch scan and concrete pass (nvc_cache_decode.cuh)
+cudaError_t launch_decode_indices(const IndexDecodeArgs& a, cudaStream_t stream)
+{
+	if (a.chunks == 0)
+		return cudaSuccess;
+	const uint32_t grid = (a.chunks + cache::kIndexThreads - 1) / cache::kIndexThreads;
+	const uint32_t scan_grid = (a.runs + cache::kIndexScanWarps - 1) / cache::kIndexScanWarps;
+	void (*symbolic)(IndexDecodeArgs) = cache::decode_index_symbolic_kernel;
+	void (*totals)(IndexDecodeArgs) = cache::decode_index_scan_kernel<false>;
+	void (*runs)(IndexDecodeArgs) = cache::decode_index_runs_kernel;
+	void (*prefix)(IndexDecodeArgs) = cache::decode_index_scan_kernel<true>;
+	void (*concrete)(IndexDecodeArgs) = cache::decode_index_concrete_kernel;
+	symbolic<<<grid, cache::kIndexThreads, 0, stream>>>(a);
+	totals<<<scan_grid, cache::kIndexScanWarps * 32, 0, stream>>>(a);
+	runs<<<1, 32, 0, stream>>>(a);
+	prefix<<<scan_grid, cache::kIndexScanWarps * 32, 0, stream>>>(a);
+	concrete<<<grid, cache::kIndexThreads, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
 // nvc_scene_cache_write: the vertex codec's estimate, measure, scan and write passes (nvc_cache_encode.cuh)
 cudaError_t launch_encode_vertices(const VertexEncodeArgs& a, uint32_t stride, cudaStream_t stream)
 {

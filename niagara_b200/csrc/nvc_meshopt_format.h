@@ -5,7 +5,9 @@
 //                 host decoder accepts, and the device finds every group where the walk measured it.
 //   meshlet codec a meshlet's words and the block decoder, for the host reader (nvc_scene_cache.cpp), the device decoder
 //                 (nvc_cache_decode.cuh) and the device encoder (nvc_cache_encode.cuh), which writes what it reads back.
-//   index codec   the decoder's FIFO rings, for the host decoder and encoder (nvc_meshopt_host.h, nvc_meshopt_encode.cpp).
+//   index codec   the decoder's FIFO rings, for the host decoder and encoder (nvc_meshopt_host.h, nvc_meshopt_encode.cpp),
+//                 and the per-triangle step, for the host decoder, the host walk that cuts a stream into chunks
+//                 (nvc_meshopt_host.h) and the device decoder (nvc_cache_decode.cuh).
 #pragma once
 
 #include <stddef.h>
@@ -264,6 +266,110 @@ struct Ring16
 	}
 	uint32_t back(uint32_t n) const { return slot[(head - n) & 15u]; } // back(1) = most recent
 };
+
+NVC_CODEC_FN inline uint32_t unzigzag(uint32_t v)
+{
+	return (v >> 1) ^ (0u - (v & 1u));
+}
+
+// A varint of 7 bits per byte, low group first: it ends at the first byte below 128 or after its fifth byte, whatever
+// that byte's top bit.  `data.next(b)` gives the next data byte; false when the data has ended.
+template <typename Data>
+NVC_CODEC_FN inline bool read_varint(Data& data, uint32_t& value)
+{
+	value = 0;
+	for (int i = 0; i < 5; ++i)
+	{
+		uint32_t b;
+		if (!data.next(b))
+			return false;
+		value |= (b & 127u) << (7 * i);
+		if (b < 128u)
+			break;
+	}
+	return true;
+}
+
+// One triangle of the index codec (the format is in nvc_meshopt_host.h), for the host decoder, the host walk that finds
+// where each chunk's data starts (nvc_meshopt_host.h) and the device decoder's symbolic and concrete passes
+// (nvc_cache_decode.cuh).  The state `s` holds values of type S::Value, concrete indices or not:
+//   S::add(v, k), S::zero()         v + k mod 2^32; the value 0 (a reset `next`)
+//   s.next, s.last                  the next new vertex, the last explicit index
+//   s.vert(n), s.edge_a(n), s.edge_b(n)   ring lookups n back, 1 <= n <= 15 (1 = the most recent push)
+//   s.put_vert(v, advance), s.put_edge(a, b)
+// A FIFO hit (put_vert(v, false)) writes the head slot without advancing, and the next advancing put overwrites that slot;
+// lookups reach at most 15 back in a 16-slot ring, so nothing reads it in between.  The device decoder still tracks that
+// write, physical slot by slot, so its chunk entry states are the serial decoder's exactly.
+// Data bytes come from `data` (see read_varint).  Returns false, with the triangle unfinished, exactly where
+// decode_index_buffer finds the stream corrupt: an aux byte or a varint that runs past the data.
+template <typename S, typename Data>
+NVC_CODEC_FN inline bool decode_triangle(S& s, uint32_t code, const uint8_t* aux, uint32_t direct_slots, Data& data, typename S::Value (&corner)[3])
+{
+	if (code < 0xf0u)
+	{
+		const uint32_t e = (code >> 4) + 1u, sel = code & 15u;
+		corner[0] = s.edge_a(e);
+		corner[1] = s.edge_b(e);
+		if (sel < direct_slots)
+		{
+			corner[2] = sel == 0 ? s.next : s.vert(sel + 1u);
+			if (sel == 0)
+				s.next = S::add(s.next, 1u);
+			s.put_vert(corner[2], sel == 0);
+		}
+		else
+		{
+			uint32_t delta = sel == 13u ? 0xffffffffu : 1u; // 13 -> -1, 14 -> +1
+			if (sel == 15u && !read_varint(data, delta))
+				return false;
+			s.last = S::add(s.last, sel == 15u ? unzigzag(delta) : delta);
+			corner[2] = s.last;
+			s.put_vert(corner[2], true);
+		}
+		s.put_edge(corner[2], corner[1]);
+		s.put_edge(corner[0], corner[2]);
+		return true;
+	}
+	uint32_t sel_a = 0, x;
+	if (code < 0xfeu)
+		x = aux[code & 15u];
+	else
+	{
+		if (!data.next(x))
+			return false;
+		sel_a = code == 0xfeu ? 0u : 15u;
+		if (x == 0)
+			s.next = S::zero();
+	}
+	// each corner: the next new vertex (0), an explicit varint (15), else a vertex-ring lookup.  Lookups see the ring as
+	// it is before this triangle's pushes; `next` and the varints are consumed in corner order a, b, c.
+	const uint32_t sel[3] = { sel_a, x >> 4, x & 15u };
+	for (int j = 0; j < 3; ++j)
+	{
+		if (sel[j] == 0)
+		{
+			corner[j] = s.next;
+			s.next = S::add(s.next, 1u);
+		}
+		else if (sel[j] == 15u)
+		{
+			uint32_t delta;
+			if (!read_varint(data, delta))
+				return false;
+			s.last = S::add(s.last, unzigzag(delta));
+			corner[j] = s.last;
+		}
+		else
+			corner[j] = s.vert(sel[j]);
+	}
+	s.put_vert(corner[0], true);
+	s.put_vert(corner[1], sel[1] == 0 || sel[1] == 15u);
+	s.put_vert(corner[2], sel[2] == 0 || sel[2] == 15u);
+	s.put_edge(corner[1], corner[0]);
+	s.put_edge(corner[2], corner[1]);
+	s.put_edge(corner[0], corner[2]);
+	return true;
+}
 
 } // namespace icodec
 

@@ -281,117 +281,183 @@ inline int walk_vertex_stream(const uint8_t* stream, size_t stream_size, uint32_
 	return r.at == r.end ? NVC_OK : NVC_ERROR_CORRUPT;
 }
 
-// The index codec into index_size (2 or 4) bytes per index; 16-bit outputs keep the low half of each index
-inline int decode_index_buffer(const uint8_t* stream, size_t stream_size, uint32_t index_count, uint32_t index_size, void* out)
+// Data bytes of an index stream for icodec::decode_triangle: those between the code bytes and the aux table
+struct IndexData
 {
-	if (index_count % 3 != 0 || (index_size != 2 && index_size != 4))
+	mhost::ByteReader r;
+	bool next(uint32_t& b)
+	{
+		const uint8_t* p;
+		if (!r.take(1, p))
+			return false;
+		b = *p;
+		return true;
+	}
+};
+
+// The index codec's decoder state over concrete indices (icodec::decode_triangle)
+struct IndexState
+{
+	using Value = uint32_t;
+	icodec::Ring16 verts, edges_a, edges_b;
+	uint32_t next = 0, last = 0;
+	static uint32_t add(uint32_t v, uint32_t k) { return v + k; }
+	static uint32_t zero() { return 0; }
+	uint32_t vert(uint32_t n) const { return verts.back(n); }
+	uint32_t edge_a(uint32_t n) const { return edges_a.back(n); }
+	uint32_t edge_b(uint32_t n) const { return edges_b.back(n); }
+	void put_vert(uint32_t v, bool advance) { verts.put(v, advance); }
+	void put_edge(uint32_t a, uint32_t b)
+	{
+		edges_a.put(a);
+		edges_b.put(b);
+	}
+};
+
+// The header checks of an index stream of index_count indices: its version, or a negative NvcStatus
+inline int open_index_stream(const uint8_t* stream, size_t stream_size, uint32_t index_count)
+{
+	if (index_count % 3 != 0)
 		return NVC_ERROR_INVALID_ARGUMENT;
-	const uint32_t triangles = index_count / 3;
-	if (stream_size < size_t(1) + triangles + 16)
+	if (stream_size < size_t(1) + index_count / 3 + 16)
 		return NVC_ERROR_CORRUPT;
 	if ((stream[0] & 0xf0) != 0xe0)
 		return NVC_ERROR_CORRUPT;
 	const int version = stream[0] & 0x0f;
-	if (version > 1)
-		return NVC_ERROR_UNSUPPORTED;
-	const uint32_t direct_slots = version >= 1 ? 13u : 15u;
+	return version > 1 ? NVC_ERROR_UNSUPPORTED : version;
+}
 
+// code < 0xf0 with c = low nibble: FIFO slots below this, then last -/+ 1 (v1) and the explicit varint
+inline uint32_t index_direct_slots(int version)
+{
+	return version >= 1 ? 13u : 15u;
+}
+
+// The index codec into index_size (2 or 4) bytes per index; 16-bit outputs keep the low half of each index
+inline int decode_index_buffer(const uint8_t* stream, size_t stream_size, uint32_t index_count, uint32_t index_size, void* out)
+{
+	if (index_size != 2 && index_size != 4)
+		return NVC_ERROR_INVALID_ARGUMENT;
+	const int version = open_index_stream(stream, stream_size, index_count);
+	if (version < 0)
+		return version;
+	const uint32_t triangles = index_count / 3, direct_slots = index_direct_slots(version);
 	const uint8_t* codes = stream + 1;
 	const uint8_t* aux = stream + stream_size - 16;
-	mhost::ByteReader r = { codes + triangles, aux };
-
-	icodec::Ring16 verts, edge_a, edge_b;
-	auto push_edge = [&](uint32_t a, uint32_t b) {
-		edge_a.put(a);
-		edge_b.put(b);
-	};
-	uint32_t next = 0, last = 0;
-
+	IndexData data = { { codes + triangles, aux } };
+	IndexState s;
 	for (uint32_t t = 0; t < triangles; ++t)
 	{
-		const uint32_t code = codes[t];
-		uint32_t a, b, c;
-		if (code < 0xf0)
-		{
-			uint32_t e = (code >> 4) + 1u;
-			a = edge_a.back(e);
-			b = edge_b.back(e);
-			uint32_t sel = code & 15u;
-			if (sel < direct_slots)
-			{
-				c = sel == 0 ? next : verts.back(sel + 1u);
-				next += sel == 0 ? 1u : 0u;
-				verts.put(c, sel == 0);
-			}
-			else
-			{
-				if (sel == 15u)
-				{
-					if (!mhost::read_varint_delta(r, last))
-						return NVC_ERROR_CORRUPT;
-				}
-				else
-					last += sel == 13u ? 0xffffffffu : 1u; // 13 -> -1, 14 -> +1
-				c = last;
-				verts.put(c);
-			}
-			push_edge(c, b);
-			push_edge(a, c);
-		}
-		else
-		{
-			uint32_t sel_a = 0, sel_b, sel_c;
-			if (code < 0xfe)
-			{
-				uint32_t x = aux[code & 15u];
-				sel_b = x >> 4;
-				sel_c = x & 15u;
-			}
-			else
-			{
-				const uint8_t* x;
-				if (!r.take(1, x))
-					return NVC_ERROR_CORRUPT;
-				sel_a = code == 0xfe ? 0u : 15u;
-				sel_b = *x >> 4;
-				sel_c = *x & 15u;
-				if (*x == 0)
-					next = 0;
-			}
-			// FIFO lookups use the ring as it is BEFORE this triangle's vertices are pushed
-			a = sel_a == 0 ? next++ : 0u;
-			b = sel_b == 0 ? next++ : verts.back(sel_b);
-			c = sel_c == 0 ? next++ : verts.back(sel_c);
-			if (sel_a == 15u)
-			{
-				if (!mhost::read_varint_delta(r, last))
-					return NVC_ERROR_CORRUPT;
-				a = last;
-			}
-			if (sel_b == 15u)
-			{
-				if (!mhost::read_varint_delta(r, last))
-					return NVC_ERROR_CORRUPT;
-				b = last;
-			}
-			if (sel_c == 15u)
-			{
-				if (!mhost::read_varint_delta(r, last))
-					return NVC_ERROR_CORRUPT;
-				c = last;
-			}
-			verts.put(a);
-			verts.put(b, sel_b == 0 || sel_b == 15u);
-			verts.put(c, sel_c == 0 || sel_c == 15u);
-			push_edge(b, a);
-			push_edge(c, b);
-			push_edge(a, c);
-		}
-		mhost::store_index(out, size_t(t) * 3 + 0, index_size, a);
-		mhost::store_index(out, size_t(t) * 3 + 1, index_size, b);
-		mhost::store_index(out, size_t(t) * 3 + 2, index_size, c);
+		uint32_t corner[3];
+		if (!icodec::decode_triangle(s, codes[t], aux, direct_slots, data, corner))
+			return NVC_ERROR_CORRUPT;
+		mhost::store_index(out, size_t(t) * 3 + 0, index_size, corner[0]);
+		mhost::store_index(out, size_t(t) * 3 + 1, index_size, corner[1]);
+		mhost::store_index(out, size_t(t) * 3 + 2, index_size, corner[2]);
 	}
-	return r.at == r.end ? NVC_OK : NVC_ERROR_CORRUPT;
+	return data.r.at == data.r.end ? NVC_OK : NVC_ERROR_CORRUPT;
+}
+
+// A decoder state that holds nothing: icodec::decode_triangle over it only consumes data bytes
+struct IndexShape
+{
+	struct Value
+	{
+	};
+	Value next, last;
+	static Value add(Value, uint32_t) { return Value(); }
+	static Value zero() { return Value(); }
+	Value vert(uint32_t) const { return Value(); }
+	Value edge_a(uint32_t) const { return Value(); }
+	Value edge_b(uint32_t) const { return Value(); }
+	void put_vert(Value, bool) {}
+	void put_edge(Value, Value) {}
+};
+
+// A data source that counts the bytes the step reads: the first is `first`, every later one ends a varint
+struct IndexTokenCounter
+{
+	uint32_t first, reads;
+	bool next(uint32_t& b)
+	{
+		b = reads++ == 0 ? first : 0u;
+		return true;
+	}
+};
+
+// Skips `count` varints from `at`; false when one runs past `end` (icodec::read_varint's rule: a varint ends at its first
+// byte below 128 or after its fifth byte)
+inline bool skip_varints(const uint8_t*& at, const uint8_t* end, uint32_t count)
+{
+	for (; count; --count)
+		for (int i = 0;; ++i)
+		{
+			if (at == end)
+				return false;
+			if (*at++ < 128u || i == 4)
+				break;
+		}
+	return true;
+}
+
+// Cuts an index stream into chunks of `chunk` triangles for the device decoder (nvc_cache_decode.cuh) without decoding
+// it: chunk_data[c] = the offset from the stream's start of the first data byte triangle c * chunk reads, for every
+// chunk c.  Only code bytes, the aux bytes of 0xfe / 0xff and the ends of varints are read.  How many varints a triangle
+// holds comes from the decoder's own step (icodec::decode_triangle over a state that holds nothing), tabled per code
+// and per aux byte, and the walk reads the data bytes in the decoder's order, so it returns the status
+// decode_index_buffer returns on every stream, and a stream it accepts decodes on the device without a check.  Returns
+// the version (0 or 1), or a negative NvcStatus.
+inline int walk_index_stream(const uint8_t* stream, size_t stream_size, uint32_t index_count, uint32_t chunk, uint64_t* chunk_data)
+{
+	const int version = open_index_stream(stream, stream_size, index_count);
+	if (version < 0)
+		return version;
+	const uint32_t triangles = index_count / 3, direct_slots = index_direct_slots(version);
+	const uint8_t* codes = stream + 1;
+	const uint8_t* aux = stream + stream_size - 16;
+	// varints of a triangle by its code (below 0xfe), and after the aux byte x of 0xfe / 0xff
+	uint8_t varints[256], varints_after[2][256];
+	IndexShape s;
+	IndexShape::Value corner[3];
+	for (uint32_t code = 0; code < 256; ++code)
+	{
+		IndexTokenCounter count = { 0, 0 };
+		if (code < 0xfe)
+			icodec::decode_triangle(s, code, aux, direct_slots, count, corner);
+		varints[code] = uint8_t(count.reads);
+	}
+	for (uint32_t x = 0; x < 256; ++x)
+		for (uint32_t k = 0; k < 2; ++k)
+		{
+			IndexTokenCounter count = { x, 0 };
+			icodec::decode_triangle(s, 0xfe + k, aux, direct_slots, count, corner);
+			varints_after[k][x] = uint8_t(count.reads - 1);
+		}
+	const uint8_t* at = codes + triangles;
+	uint32_t pending = 0; // varints to skip before the next aux byte or chunk start
+	for (uint32_t first = 0, c = 0; first < triangles; first += chunk, ++c)
+	{
+		if (!skip_varints(at, aux, pending))
+			return NVC_ERROR_CORRUPT;
+		pending = 0;
+		chunk_data[c] = uint64_t(at - stream);
+		const uint32_t end = triangles - first < chunk ? triangles : first + chunk;
+		for (uint32_t t = first; t < end; ++t)
+		{
+			const uint32_t code = codes[t];
+			if (code < 0xfe)
+				pending += varints[code];
+			else
+			{
+				if (!skip_varints(at, aux, pending) || at == aux)
+					return NVC_ERROR_CORRUPT;
+				pending = varints_after[code & 1][*at++];
+			}
+		}
+	}
+	if (!skip_varints(at, aux, pending))
+		return NVC_ERROR_CORRUPT;
+	return at == aux ? version : NVC_ERROR_CORRUPT;
 }
 
 inline int decode_index_stream(const uint8_t* stream, size_t stream_size, uint32_t index_count, uint32_t* out)

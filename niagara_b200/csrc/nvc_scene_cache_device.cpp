@@ -1,7 +1,7 @@
-// nvc_scene_cache_device.cpp — nvc_scene_cache_read into device memory.  The vertex streams (VERTICES, MESHLETVTX0) and
-// the per-meshlet stream (MESHLETDATA) go up as stored, with an index the host finds by walking their sizes only
-// (walk_vertex_stream, index_meshlet_stream), and are decoded by the kernels of nvc_cache_decode.cuh.  Raw sections are
-// copied up; INDICES is decoded on the host (the index codec is one sequential FIFO state machine) and copied up.
+// nvc_scene_cache_device.cpp — nvc_scene_cache_read into device memory.  The vertex streams (VERTICES, MESHLETVTX0), the
+// per-meshlet stream (MESHLETDATA) and the index stream (INDICES) go up as stored, with an index the host finds by walking
+// their sizes only (walk_vertex_stream, index_meshlet_stream, walk_index_stream), and are decoded by the kernels of
+// nvc_cache_decode.cuh.  Raw sections are copied up.
 #include "nvc_internal.h"
 #include "nvc_meshopt_host.h"
 
@@ -102,6 +102,44 @@ int read_meshletdata(NvcContext* ctx, cudaStream_t stream, const void* file, siz
 	return corrupt ? NVC_ERROR_CORRUPT : NVC_OK;
 }
 
+int read_indices(NvcContext* ctx, cudaStream_t stream, const uint8_t* data, const NvcSceneCacheSection& sec, void* dst)
+{
+	const uint32_t triangles = sec.count / 3, chunks = (triangles + nvc::kIndexChunk - 1) / nvc::kIndexChunk;
+	const uint32_t runs = (chunks + nvc::kIndexRun - 1) / nvc::kIndexRun;
+	std::vector<uint64_t> chunk_data(chunks);
+	const int version = nvc::walk_index_stream(data, sec.stored_bytes, sec.count, nvc::kIndexChunk, chunk_data.data());
+	if (version < 0)
+		return version;
+	if (chunks == 0)
+		return NVC_OK;
+
+	nvc::ScratchPlan plan; // the staged stream is taken last: a scratch allocated for this call ends where its last word does
+	const size_t o_data = plan.take(chunk_data.size() * 8), o_sub = plan.take(size_t(chunks) * nvc::kIndexEntries * 8);
+	const size_t o_run = plan.take(size_t(runs) * nvc::kIndexEntries * 8), o_stream = plan.take(staged_bytes(sec.stored_bytes));
+	cudaError_t e = nvc::reserve_scratch(ctx, plan.bytes);
+	char* base = static_cast<char*>(ctx->load_scratch);
+	if (e == cudaSuccess)
+		e = nvc::upload({ { base + o_stream, data, sec.stored_bytes }, { base + o_data, chunk_data.data(), chunk_data.size() * 8 } });
+	if (e != cudaSuccess)
+		return nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
+
+	nvc::IndexDecodeArgs a;
+	a.stream = reinterpret_cast<const uint8_t*>(base + o_stream);
+	a.chunk_data = reinterpret_cast<const uint64_t*>(base + o_data);
+	a.sub = reinterpret_cast<uint2*>(base + o_sub);
+	a.run = reinterpret_cast<uint2*>(base + o_run);
+	a.out = static_cast<uint32_t*>(dst);
+	a.aux_offset = sec.stored_bytes - 16;
+	a.triangles = triangles;
+	a.chunks = chunks;
+	a.runs = runs;
+	a.direct_slots = nvc::index_direct_slots(version);
+	e = nvc::launch_decode_indices(a, stream);
+	if (e == cudaSuccess)
+		e = cudaDeviceSynchronize();
+	return e == cudaSuccess ? NVC_OK : nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
+}
+
 } // namespace
 
 extern "C" NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream, const void* file, size_t file_size, const NvcSceneCacheInfo* info, int section, void* dst,
@@ -129,7 +167,8 @@ extern "C" NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream
 		e = nvc::upload({ { dst, data, sec.decoded_bytes } });
 		return e == cudaSuccess ? NVC_OK : nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
 	}
-	// the kernels and their index address the staged stream with 32-bit offsets
+	// the vertex and meshlet kernels and their indexes address the staged stream with 32-bit offsets (the index kernels' chunk
+	// offsets are 64-bit: a triangle takes up to 15 data bytes)
 	if (section != NVC_CACHE_INDICES && sec.stored_bytes > 0xffffffffull)
 		return NVC_ERROR_UNSUPPORTED;
 	if (section == NVC_CACHE_VERTICES)
@@ -137,14 +176,7 @@ extern "C" NVC_API int nvc_scene_cache_read_device(NvcContext* ctx, void* stream
 	if (section == NVC_CACHE_MESHLETVTX0) // uint16 x 4 per element of the stream
 		return sec.count % 4 ? NVC_ERROR_CORRUPT : read_vertices(ctx, s, data, sec, sec.count / 4, 8, dst);
 	if (section == NVC_CACHE_INDICES)
-	{
-		std::vector<uint32_t> indices(sec.count);
-		int status = nvc::decode_index_stream(data, sec.stored_bytes, sec.count, indices.data());
-		if (status != NVC_OK)
-			return status;
-		e = nvc::upload({ { dst, indices.data(), sec.decoded_bytes } });
-		return e == cudaSuccess ? NVC_OK : nvc::load_fail(ctx, e, "nvc_scene_cache_read_device");
-	}
+		return read_indices(ctx, s, data, sec, dst);
 	if (section != NVC_CACHE_MESHLETDATA)
 		return NVC_ERROR_UNSUPPORTED;
 	return read_meshletdata(ctx, s, file, file_size, info, dst);

@@ -64,8 +64,8 @@ class SceneCache:
 
     def section_device(self, name, device="cuda"):
         """The section's decoded bytes as a torch.uint8 tensor on `device`, equal to `section(name)`'s bytes
-        (nvc_scene_cache_read_device: the compressed vertex streams and meshlet data go up as stored and are decoded by
-        kernels; indices are decoded on the host).  Runs on the device's current stream and synchronises the device."""
+        (nvc_scene_cache_read_device: the compressed vertex streams, indices and meshlet data go up as stored and are
+        decoded by kernels).  Runs on the device's current stream and synchronises the device."""
         import torch
 
         idx = layout.CACHE_SECTIONS.index(name)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Times reading a compressed scene cache's VERTICES and MESHLETDATA sections into device memory two ways:
+"""Times reading a compressed scene cache's VERTICES, INDICES and MESHLETDATA sections into device memory two ways:
 
   (a) host   nvc_scene_cache_read into pinned host memory, then one copy up, ending in a synchronise
   (b) device nvc_scene_cache_read_device: the stream goes up as stored and is decoded by kernels; its host walk (the
@@ -8,7 +8,8 @@
 Workload: --copies copies of tests/golden/kitten.z.cache's geometry in one cache, from --seed: the vertices with seeded
 jitter in the fp16 positions, re-encoded with the reference's vertex encoder at level 2 (as writeVertexCompressed does;
 oracle/_ref/libmeshopt_ref.so, required); Meshlet[] with per-copy data offsets; the meshlet blocks copied verbatim
-(references are mesh-local).  Both outputs are compared in the same run.  Times: host clock around each call (every
+(references are mesh-local); kitten's index chain (every LOD) repeated per copy, re-encoded with the reference's index
+encoder at the stream's own version (as saveSceneCache writes it).  Both outputs are compared in the same run.  Times: host clock around each call (every
 call ends in a device synchronise), median of --iters calls after --warmup.  Prints the card, its power limit and max SM
 clock, and one JSON line.
 
@@ -30,8 +31,8 @@ REF_SO = os.path.join(ROOT, "oracle", "_ref", "libmeshopt_ref.so")
 HEADER = 160
 
 
-def generate(copies=1000, seed=1):
-    """the workload cache as a uint8 array"""
+def generate(copies=1000, seed=1, indices=False):
+    """the workload cache as a uint8 array; with `indices`, an INDICES section too"""
     from niagara_b200 import layout
     from niagara_b200.lib import load_library
 
@@ -76,15 +77,30 @@ def generate(copies=1000, seed=1):
     all_meshlets["dataOffset"] += (np.arange(copies, dtype=np.uint32) * words).repeat(len(meshlets))
     chain = np.tile(stored("meshletdata"), copies)
 
+    istream = np.zeros(0, np.uint8)
+    index_count = 0
+    if indices:
+        ichain = np.ascontiguousarray(np.tile(read("indices").view(np.uint32), copies))
+        ref.meshopt_encodeIndexVersion.argtypes = [ctypes.c_int]
+        ref.meshopt_encodeIndexBufferBound.restype = ctypes.c_size_t
+        ref.meshopt_encodeIndexBufferBound.argtypes = [ctypes.c_size_t, ctypes.c_size_t]
+        ref.meshopt_encodeIndexBuffer.restype = ctypes.c_size_t
+        ref.meshopt_encodeIndexBuffer.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]
+        ref.meshopt_encodeIndexVersion(int(stored("indices")[0]) & 15)
+        ibuf = np.zeros(ref.meshopt_encodeIndexBufferBound(len(ichain), int(ichain.max()) + 1), np.uint8)
+        m = ref.meshopt_encodeIndexBuffer(ibuf.ctypes.data, len(ibuf), ichain.ctypes.data, len(ichain))
+        assert m > 0
+        istream, index_count = ibuf[:m], len(ichain)
+
     h = layout.SceneCacheHeader.from_buffer_copy(src[:HEADER].tobytes())
     h.compressed = 1
     h.vertexCount, h.compressedVertexBytes = len(many), n
-    h.indexCount = h.compressedIndexBytes = 0
+    h.indexCount, h.compressedIndexBytes = index_count, len(istream)
     h.meshletCount, h.meshletdataCount, h.compressedMeshletDataBytes = len(all_meshlets), words * copies, len(chain)
     for field in ("meshletvtx0Count", "compressedMeshletVtx0Bytes", "meshCount", "materialCount", "drawCount", "texturePathCount", "lightCount",
                   "animationCount", "keyframeCount", "ommArrayDataSize", "ommIndexDataSize", "ommDescCount"):
         setattr(h, field, 0)
-    return np.concatenate([np.frombuffer(bytes(h), np.uint8), vstream, all_meshlets.view(np.uint8), chain])
+    return np.concatenate([np.frombuffer(bytes(h), np.uint8), vstream, istream, all_meshlets.view(np.uint8), chain])
 
 
 def card():
@@ -117,7 +133,7 @@ def main():
     assert torch.cuda.is_available(), "the benchmark needs a CUDA device"
     lib = load_library()
     t0 = time.perf_counter()
-    data = generate(args.copies, args.seed)
+    data = generate(args.copies, args.seed, indices=True)
     print("generated %d copies in %.1f s" % (args.copies, time.perf_counter() - t0), flush=True)
     info = layout.SceneCacheInfo()
     assert lib.nvc_scene_cache_parse(data.ctypes.data, len(data), ctypes.byref(info)) == 0
@@ -125,7 +141,7 @@ def main():
     check(lib.nvc_create(0, None, ctypes.byref(ctx)), None, "nvc_create")
     stream = torch.cuda.current_stream().cuda_stream
     results = {"card": card(), "copies": args.copies, "seed": args.seed, "iters": args.iters}
-    for name in ("vertices", "meshletdata"):
+    for name in ("vertices", "indices", "meshletdata"):
         s = layout.CACHE_SECTIONS.index(name)
         sec = info.sections[s]
         n = int(sec.decoded_bytes)
@@ -163,6 +179,7 @@ def main():
         walks = walk_times(path, args.iters)
     results["vertices"]["host_walk_ms"] = walks["vertices_walk_ms"]
     results["meshletdata"]["host_walk_ms"] = walks["meshletdata_walk_ms"]
+    results["indices"]["host_walk_ms"] = walks["indices_walk_ms"]
     print(json.dumps(results))
 
 

@@ -1,6 +1,6 @@
-// Times the host walks of nvc_scene_cache_read_device on their own: walk_vertex_stream over VERTICES and
-// index_meshlet_stream over MESHLETDATA, the serial part of the device read.  Built from the library's host sources by
-// tools/scene_cache_device_bench.py.  Usage: scene_cache_walk_timer <file.cache> <iterations>; prints one JSON line with
+// Times the host walks of nvc_scene_cache_read_device on their own: walk_vertex_stream over VERTICES,
+// walk_index_stream over INDICES and index_meshlet_stream over MESHLETDATA, the serial part of the device read.  Built
+// from the library's host sources by tools/scene_cache_device_bench.py.  Usage: scene_cache_walk_timer <file.cache> <iterations>; prints one JSON line with
 // the median milliseconds of each walk.
 #include "nvc_meshopt_host.h"
 
@@ -17,7 +17,7 @@ static double median_ms(int iterations, F&& f)
 	for (int i = 0; i < iterations; ++i)
 	{
 		auto t0 = std::chrono::steady_clock::now();
-		if (f() != NVC_OK)
+		if (f() < 0)
 		{
 			fprintf(stderr, "walk failed\n");
 			exit(1);
@@ -53,6 +53,10 @@ int main(int argc, char** argv)
 	const uint32_t meshlets = info.header.meshletCount;
 	std::vector<uint32_t> checkpoints((meshlets + nvc::kMeshletGroup - 1) / nvc::kMeshletGroup + 1), records(size_t(meshlets) * 2);
 	double meshlet_ms = median_ms(iterations, [&] { return nvc::index_meshlet_stream(file.data(), file.size(), &info, checkpoints.data(), records.data()); });
-	printf("{\"vertices_walk_ms\": %.3f, \"meshletdata_walk_ms\": %.3f}\n", vertex_ms, meshlet_ms);
+	const NvcSceneCacheSection& x = info.sections[NVC_CACHE_INDICES];
+	const uint32_t chunk = 256; // the device decoder's kIndexChunk (nvc_internal.h)
+	std::vector<uint64_t> chunk_data((x.count / 3 + chunk - 1) / chunk);
+	double index_ms = x.count ? median_ms(iterations, [&] { return nvc::walk_index_stream(file.data() + x.offset, x.stored_bytes, x.count, chunk, chunk_data.data()); }) : 0.0;
+	printf("{\"vertices_walk_ms\": %.3f, \"indices_walk_ms\": %.3f, \"meshletdata_walk_ms\": %.3f}\n", vertex_ms, index_ms, meshlet_ms);
 	return 0;
 }
