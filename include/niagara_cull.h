@@ -234,6 +234,9 @@ NVC_API int nvc_set_cluster_filter(NvcContext* ctx, int enabled);
 /* Diagnostics (synchronises the device): out[0] = meshlets the filtered cluster passes evaluated, out[1] = how many of them
  * were undecided and took the exact path, both cumulative since the last call with reset != 0. */
 NVC_API int nvc_filter_stats(NvcContext* ctx, uint64_t* out_items_undecided2, int reset);
+/* Diagnostics / tests: enqueues on `stream` the filter's approximate reciprocal (op 0) or square root (op 1) of n float bit
+ * patterns: out[i] = bits of op(float bits in[i]), as the filtered cluster pass computes them (device arrays of n uint32). */
+NVC_API int nvc_filter_approx(NvcContext* ctx, void* stream, int op, const uint32_t* in, uint32_t* out, uint64_t n);
 
 /* ---- pyramid layout (host only): niagara.cpp:439-447 previousPow2, resources.cpp:280-292 getImageMipLevels,
  *      niagara.cpp:1339-1342 ------------------------------------------------------------------------- */

@@ -349,6 +349,16 @@ NVC_API int nvc_filter_stats(NvcContext* ctx, uint64_t* out_items_undecided2, in
 	return NVC_OK;
 }
 
+NVC_API int nvc_filter_approx(NvcContext* ctx, void* stream, int op, const uint32_t* in, uint32_t* out, uint64_t n)
+{
+	if (!ctx || (op != 0 && op != 1) || (n && (!in || !out)) || n > (uint64_t(INT32_MAX) << 8)) // one 256-thread block per 256 inputs
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	cudaError_t e = nvc::launch_filter_approx(in, out, n, op, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_filter_approx");
+}
+
 NVC_API int nvc_drawcull(NvcContext* ctx, void* stream, const NvcCullData* cull, int late, int task,
     const NvcMeshDraw* draws, const NvcMesh* meshes, uint32_t* draw_visibility,
     void* commands, uint32_t* command_count4, const NvcHiZ* hiz)

@@ -39,10 +39,18 @@
 //     fract(x) is within efp of 0 / 1 (this includes the fract == 0 special case of the sampler).  Decided items read
 //     exactly the texels the exact path reads, so `depth` is the same float.
 // (7) depthSphere = znear / (cz - r) differs by <= 1.7 relE depthSphere -> margin 2 relE depthSphere.
+// (8) rcp.approx.ftz / sqrt.approx.ftz are within a relative 2^-22 of the true value only where argument and result are
+//     normal: a subnormal argument is read as 0 and a subnormal result written as 0 (100 % error), and below ~2^-126 the
+//     other products round with an absolute, not relative, error of 2^-150 that (1)-(7) do not budget.  The root of the
+//     cone test and the shared reciprocal of (4) therefore decide only when their argument lies in [2^-110, 2^110]:
+//     |c|^2 >= 2^-110 for the cone; c.z^2 - r^2 in [2^-110, 2^110] for the occlusion stage (then c.x^2 + c.z^2 - r^2 is
+//     normal too, and c.z - r >= znear > 1e-30 is required anyway).  Inside that range every subnormal rounding is below
+//     2^-40 relative to what it perturbs; the rest of the cone and the frustum are covered by the 2^-100 floor of E.
 // Non-finite or out-of-range inputs never produce a decision: every "sure" predicate is a strict comparison that is
 // false for NaN, commands with unusual transforms are flagged exact-only in build_record, and integer conversions are
 // clamped first.  tests/filter_harness.cpp checks 10^8+ random / hostile items against the exact path with the MUFU
-// results perturbed by +-2 ulp, and checks the margins against a float64 evaluation.
+// results perturbed by +-2 ulp and flushed as the device flushes them, and checks the margins against a float64
+// evaluation; tests/test_filter_approx.py compares both instructions on the H100 with float64 over all 2^32 inputs.
 #pragma once
 
 #include "nvc_internal.h"
@@ -55,7 +63,9 @@ namespace nvc
 {
 
 #if defined(NVC_EMU)
-// CPU stand-ins; NVF_PERTURB (tests) scales every approximate reciprocal / root by 1 +- 2^-22 pseudo-randomly
+// CPU stand-ins with the special-value rules of the .ftz instructions: a subnormal argument is read as a zero of its sign, a
+// subnormal result is written as one, NaN results are the canonical 0x7fffffff, sqrt(-0) = -0 and sqrt(x < 0) = NaN.
+// NVF_PERTURB (tests) scales every normal result by 1 +- 2^-22 pseudo-randomly (the relative error budget of both instructions).
 #ifdef NVF_PERTURB
 extern thread_local uint32_t nvf_perturb_state;
 __device__ __forceinline__ float nvf_jitter(float v)
@@ -68,8 +78,21 @@ __device__ __forceinline__ float nvf_jitter(float v)
 #else
 __device__ __forceinline__ float nvf_jitter(float v) { return v; }
 #endif
-__device__ __forceinline__ float nvf_rcp(float x) { return nvf_jitter(1.0f / x); }
-__device__ __forceinline__ float nvf_sqrt(float x) { return nvf_jitter(sqrtf(x)); }
+__device__ __forceinline__ float nvf_ftz(float x)
+{
+	return (__float_as_uint(x) & 0x7f800000u) == 0u ? __uint_as_float(__float_as_uint(x) & 0x80000000u) : x;
+}
+__device__ __forceinline__ float nvf_result(float v)
+{
+	const uint32_t e = __float_as_uint(v) & 0x7f800000u;
+	if (v != v)
+		return __uint_as_float(0x7fffffffu);
+	if (e == 0u)
+		return nvf_ftz(v);
+	return e == 0x7f800000u ? v : nvf_jitter(v);
+}
+__device__ __forceinline__ float nvf_rcp(float x) { return nvf_result(1.0f / nvf_ftz(x)); }
+__device__ __forceinline__ float nvf_sqrt(float x) { return nvf_result(sqrtf(nvf_ftz(x))); }
 #else
 __device__ __forceinline__ float nvf_rcp(float x)
 {
@@ -86,6 +109,10 @@ __device__ __forceinline__ float nvf_sqrt(float x)
 #endif
 
 __device__ __forceinline__ float nvf_fma(float a, float b, float c) { return __fmaf_rn(a, b, c); }
+
+// Error model (8): the range of arguments of nvf_rcp / nvf_sqrt in which a decision may be taken
+constexpr float kNvfMinArg = 7.7037198e-34f; // 2^-110
+constexpr float kNvfMaxArg = 1.2980742e33f;  // 2^110
 
 // Host side: the per-launch constants from the pass's CullData and pyramid (called by nvc_clustercull, nvc_api.cu).
 // Anything unusual (non-finite view, huge row sums, non-positive projection scale, non power-of-two pyramid) switches
@@ -243,9 +270,10 @@ __device__ __forceinline__ void filter_occlusion(const FilterConsts& fc, const N
 	const float relE = E * iD;
 	const float g = nvf_fma(r, iD, 1.f);
 	const float gr = g * relE;
-	// domain of the error analysis: radius >= 0, sphere inside the validity cone, small relative uncertainty
+	// domain of the error analysis: radius >= 0, sphere inside the validity cone, small relative uncertainty, c.z^2 - r^2 far
+	// from the range where the approximate reciprocal / roots flush (then so is c.x^2 + c.z^2 - r^2 >= c.z^2 - r^2)
 	const float cone_x = nvf_fma(-fc.cg.x, cz, nvf_fma(r, fc.cg.y, fabsf(cx))), cone_y = nvf_fma(-fc.cg.z, cz, nvf_fma(r, fc.cg.w, fabsf(cy)));
-	const bool dom_ok = r >= 0.f && cone_x <= 0.f && cone_y <= 0.f && gr < 9.765625e-4f /* 2^-10 */; // (fc.occ_ok is checked by the host: nvc_clustercull)
+	const bool dom_ok = r >= 0.f && cone_x <= 0.f && cone_y <= 0.f && gr < 9.765625e-4f /* 2^-10 */ && czr2 >= kNvfMinArg && czr2 <= kNvfMaxArg; // (fc.occ_ok is checked by the host: nvc_clustercull)
 
 	const float vx = nvf_sqrt(nvf_fma(cx, cx, czr2)), vy = nvf_sqrt(nvf_fma(cy, cy, czr2));
 	const float cxz = cx * cz, cyz = cy * cz, rvx = r * vx, rvy = r * vy;
@@ -356,12 +384,14 @@ __device__ __forceinline__ FilterResult filter_meshlet(const FilterConsts& fc, c
 		const float Ay = nvf_fma(row1.x, ax, nvf_fma(row1.y, ay, row1.z * az));
 		const float Az = nvf_fma(row2.x, ax, nvf_fma(row2.y, ay, row2.z * az));
 		const float dotv = nvf_fma(cx, Ax, nvf_fma(cy, Ay, cz * Az));
-		const float len = nvf_sqrt(nvf_fma(cx, cx, nvf_fma(cy, cy, cz * cz)));
+		const float lsq = nvf_fma(cx, cx, nvf_fma(cy, cy, cz * cz));
+		const float len = nvf_sqrt(lsq);
 		const float rhs = aux.x * nvf_fma(ac, len, 127.f * r);
 		const float tc = rhs - dotv; // > 0: not back-facing
 		const float mC = (8300.f * aux.x) * E; // 64 E x 127 s (+2 %)
-		pass = pass && tc > mC;
-		fail = fail || tc < -mC;
+		const bool cone_dom = lsq >= kNvfMinArg; // the root is not flushed, and the squares' subnormal rounding is negligible
+		pass = pass && tc > mC && cone_dom;
+		fail = fail || (tc < -mC && cone_dom);
 	}
 
 	if (!LATE || !occlusion)

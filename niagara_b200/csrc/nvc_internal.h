@@ -435,6 +435,7 @@ struct MeshletEncodeArgs
 // measure, scan, write (the write pass skips the meshlets the measure pass flagged)
 cudaError_t launch_encode_meshlets(const MeshletEncodeArgs& a, cudaStream_t stream);
 cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const uint32_t* update_indices, const NvcMeshDraw* update_values, uint32_t count, cudaStream_t stream);
+cudaError_t launch_filter_approx(const uint32_t* in, uint32_t* out, uint64_t n, int op, cudaStream_t stream);
 cudaError_t launch_pack_meshes(const NvcMesh* meshes, uint32_t count, MeshCullHead* heads, float* errors, cudaStream_t stream);
 cudaError_t launch_pack_meshlets(const NvcMeshlet* meshlets, uint32_t count, uint2* sphere, uint32_t* cone, cudaStream_t stream);
 cudaError_t clustercull_occupancy(int* blocks_per_sm_early, int* blocks_per_sm_late, int* blocks_per_sm_late_staged, uint32_t stage_bytes);

@@ -3478,6 +3478,24 @@ cudaError_t launch_update_draws(NvcMeshDraw* draws, uint32_t draw_count, const u
 	return cudaGetLastError();
 }
 
+// Diagnostics: the filter's approximate reciprocal (op 0) or square root (op 1) of every input bit pattern
+__global__ void filter_approx_kernel(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, uint64_t n, int op)
+{
+	const uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+	if (i >= n)
+		return;
+	const float x = __uint_as_float(__ldg(in + i));
+	out[i] = __float_as_uint(op == 0 ? nvf_rcp(x) : nvf_sqrt(x));
+}
+
+cudaError_t launch_filter_approx(const uint32_t* in, uint32_t* out, uint64_t n, int op, cudaStream_t stream)
+{
+	if (n == 0)
+		return cudaSuccess;
+	filter_approx_kernel<<<uint32_t((n + 255u) / 256u), 256, 0, stream>>>(in, out, n, op);
+	return cudaGetLastError();
+}
+
 __global__ void pack_meshes_kernel(const NvcMesh* __restrict__ meshes, uint32_t count, MeshCullHead* __restrict__ heads, float* __restrict__ errors)
 {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -40,6 +40,7 @@ SIGNATURES = [
     ("nvc_raster_depth_tasks", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.POINTER(CullData), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p]),
     ("nvc_raster_depth_indexed", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.POINTER(CullData), c_void_p, c_void_p, ctypes.c_uint32, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, ctypes.c_uint32, c_void_p]),
     ("nvc_filter_stats", ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_uint64), ctypes.c_int]),
+    ("nvc_filter_approx", ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int, c_void_p, c_void_p, ctypes.c_uint64]),
     ("nvc_set_mesh_cull", ctypes.c_int, [c_void_p, ctypes.c_int]),
     ("nvc_mesh_cull_stats", ctypes.c_int, [c_void_p, ctypes.POINTER(ctypes.c_uint64), ctypes.c_int]),
     ("nvc_set_task_cull", ctypes.c_int, [c_void_p, ctypes.c_int]),

@@ -85,7 +85,8 @@ struct Stats
 struct Scenario
 {
 	const char* name;
-	int kind; // 0 C4-like, 1 big local coordinates (bistro-like), 2 hostile bits, 3 near the camera, 4 random camera + big world offsets
+	int kind; // 0 C4-like, 1 big local coordinates (bistro-like), 2 hostile bits, 3 near the camera, 4 random camera + big world offsets,
+	          // 5 subnormal: znear, scale and view-space magnitudes where |c|^2, c.x^2 + c.z^2 - r^2 and c.z^2 - r^2 straddle [2^-149, 2^-126)
 };
 
 static uint16_t to_half(float f)
@@ -136,16 +137,16 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 		memset(&cam, 0, sizeof(cam));
 		cam.orientation[3] = 1.f;
 		cam.fovY = float(uni(0.5, 1.6));
-		cam.znear = float(sc.kind == 3 ? uni(0.01, 0.5) : uni(0.05, 1.0));
+		cam.znear = float(sc.kind == 5 ? pow(10.0, uni(-29.9, -18.0)) : sc.kind == 3 ? uni(0.01, 0.5) : uni(0.05, 1.0));
 		double world = 0;
-		if (sc.kind == 4 || (rng() & 3) == 0)
+		if (sc.kind == 4 || sc.kind == 5 || (rng() & 3) == 0)
 		{
-			// random orientation; kind 4 also moves the whole scene far from the origin
+			// random orientation; kind 4 also moves the whole scene far from the origin, kind 5 keeps the camera within a few znear of it
 			double q[4] = { uni(-1, 1), uni(-1, 1), uni(-1, 1), uni(-1, 1) };
 			double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
 			for (int i = 0; i < 4; ++i)
 				cam.orientation[i] = float(q[i] / n);
-			world = sc.kind == 4 ? uni(0, 3000) : uni(0, 50);
+			world = sc.kind == 4 ? uni(0, 3000) : sc.kind == 5 ? 4.0 * cam.znear : uni(0, 50);
 			for (int i = 0; i < 3; ++i)
 				cam.position[i] = float(uni(-world, world));
 		}
@@ -165,7 +166,7 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 				uint32_t bw = (w + 15) / 16;
 				std::vector<float> planes(size_t(bw) * ((h + 15) / 16));
 				for (auto& p : planes)
-					p = (rng() & 3) == 0 ? 0.f : float(cd.znear / uni(2.0, 400.0));
+					p = (rng() & 3) == 0 ? 0.f : float(sc.kind == 5 ? cd.znear / pow(2.0, uni(-78.0, -55.0)) : cd.znear / uni(2.0, 400.0));
 				for (uint32_t y = 0; y < h; ++y)
 					for (uint32_t x = 0; x < w; ++x)
 						t[size_t(y) * w + x] = planes[(y / 16) * bw + x / 16];
@@ -213,6 +214,16 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 				out[j] = float(V[4 * j + 0] * v[0] + V[4 * j + 1] * v[1] + V[4 * j + 2] * v[2]);
 		};
 
+		// one wrong decision as a reproducible item (float fields as bit patterns) on stderr: camera, screen, draw, meshlet
+		auto print_case = [&](const char* check, float4 d0, float4 d1, uint2 b0, uint32_t b1, bool exact, bool got) {
+			auto fb = [](float f) { return __float_as_uint(f); };
+			fprintf(stderr,
+			    "CASE {\"scenario\": \"%s\", \"check\": \"%s\", \"camera\": [%u, %u, %u, %u, %u, %u, %u, %u, %u], \"screen\": [%u, %u], \"draw_distance\": %u, \"backface\": %d, "
+			    "\"draw\": [%u, %u, %u, %u, %u, %u, %u, %u], \"meshlet\": [%u, %u, %u], \"exact\": %d, \"filter\": %d}\n",
+			    sc.name, check, fb(cam.position[0]), fb(cam.position[1]), fb(cam.position[2]), fb(cam.orientation[0]), fb(cam.orientation[1]), fb(cam.orientation[2]), fb(cam.orientation[3]), fb(cam.fovY),
+			    fb(cam.znear), sz[0], sz[1], fb(opt.draw_distance), int(cd.clusterBackfaceEnabled), fb(d0.x), fb(d0.y), fb(d0.z), fb(d0.w), fb(d1.x), fb(d1.y), fb(d1.z), fb(d1.w), b0.x, b0.y, b1,
+			    int(exact), int(got));
+		};
 		const uint64_t frame_items = std::min<uint64_t>(items - done, 2000000);
 		const uint32_t per_draw = sc.kind == 2 ? 1 : 10;
 		const double ty = tan(cam.fovY * 0.5), tx = ty * double(sz[0]) / double(sz[1]);
@@ -220,8 +231,23 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 		{
 			// ---- one draw ----
 			float4 d0, d1;
-			double sscale;
-			if (sc.kind == 2)
+			double sscale, rho = 0;
+			if (sc.kind == 5)
+			{
+				// view-space distance rho in [2^-77, 2^-50]: |c|^2 from below 2^-149 to above the filter's 2^-110 (nvc_filter.cuh (8)),
+				// mostly inside the frustum, some beside or behind the eye
+				rho = pow(2.0, uni(-77.0, -50.0));
+				double v[3] = { uni(-1, 1) * tx * 1.15, uni(-1, 1) * ty * 1.15, (rng() & 7) ? 1.0 : uni(-1, 1) };
+				const double vn = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+				float pos[3];
+				to_world(rho * v[0] / vn, rho * v[1] / vn, rho * v[2] / vn, pos);
+				sscale = pow(2.0, uni(-39.99, -30.0));
+				double q[4] = { uni(-1, 1), uni(-1, 1), uni(-1, 1), uni(-1, 1) };
+				const double qn = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+				d1 = make_float4(float(q[0] / qn), float(q[1] / qn), float(q[2] / qn), float(q[3] / qn));
+				d0 = make_float4(pos[0], pos[1], pos[2], float(sscale));
+			}
+			else if (sc.kind == 2)
 			{
 				// hostile: arbitrary bit patterns in a third of the cases, wild magnitudes otherwise
 				auto wild = [&]() -> float {
@@ -281,11 +307,20 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 					double rr = sc.kind == 1 ? uni(0.05, 3.0) : 0.02 + 0.43 * pow(U(rng), 4.0);
 					if ((rng() & 63) == 0)
 						rr = 0.0;
+					if (sc.kind == 5)
+					{
+						// local offsets of the order of rho (often 0); radius 0, an fp16 subnormal, a small normal or of the order of rho
+						const double lr = rho / sscale;
+						for (int j = 0; j < 3; ++j)
+							c[j] = (rng() & 1) ? 0.f : float(uni(-2, 2) * lr);
+						const uint32_t rk = uint32_t(rng() & 3);
+						rr = rk == 0 ? 0.0 : rk == 1 ? pow(2.0, uni(-24.0, -14.0)) : rk == 2 ? pow(2.0, uni(-14.0, -6.0)) : lr * pow(2.0, uni(-8.0, 0.5));
+					}
 					b0.x = to_half(c[0]) | (uint32_t(to_half(c[1])) << 16);
 					b0.y = to_half(c[2]) | (uint32_t(to_half(float(rr))) << 16);
 					double a[3] = { uni(-1, 1), uni(-1, 1), uni(-1, 1) };
 					double an = sqrt(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]) + 1e-9;
-					int cut = (rng() % 16 == 0) ? 127 : int(rng() % 112) + 16;
+					int cut = sc.kind == 5 ? int(int8_t(uint8_t(rng()))) : (rng() % 16 == 0) ? 127 : int(rng() % 112) + 16;
 					b1 = uint32_t(uint8_t(int8_t(lrint(a[0] / an * 127)))) | (uint32_t(uint8_t(int8_t(lrint(a[1] / an * 127)))) << 8) | (uint32_t(uint8_t(int8_t(lrint(a[2] / an * 127)))) << 16) |
 					     (uint32_t(uint8_t(int8_t(cut))) << 24);
 				}
@@ -308,7 +343,10 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 					FilterDebug keep = dbg;
 					FilterResult fq = filter_meshlet<true, true>(fc, cd, hiz, rec.row0, rec.row1, rec.row2, rec.aux, b0, b1, cd.clusterBackfaceEnabled != 0, cd.clusterOcclusionEnabled == 1);
 					if (fq.decided && fq.visible != ve) // (the jitter differs between the two calls, so `decided` may differ)
-						++st.wrong;
+					{
+						if (++st.wrong < 5)
+							print_case("footprint", d0, d1, b0, b1, ve, fq.visible);
+					}
 					dbg = keep;
 				}
 				if (!fr.decided)
@@ -325,8 +363,11 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 				{
 					++st.wrong;
 					if (st.wrong < 5)
+					{
 						fprintf(stderr, "MISMATCH %s: exact %d filter %d  c=(%g %g %g) r=%g E=%g aabb_e=(%g %g %g %g) aabb_a=(%g %g %g %g) level %d stage %d\n", sc.name, int(ve), int(fr.visible), dbg.c[0], dbg.c[1],
 						    dbg.c[2], dbg.r, dbg.E, ae[0], ae[1], ae[2], ae[3], dbg.aabb[0], dbg.aabb[1], dbg.aabb[2], dbg.aabb[3], dbg.level, dbg.stage);
+						print_case("filter", d0, d1, b0, b1, ve, fr.visible);
+					}
 				}
 				// ---- the drawcull use of the occlusion stage: exact centre, rounding-only error scale ----
 				if (ce[0] == ce[0] && ce[1] == ce[1] && ce[2] == ce[2])
@@ -350,7 +391,10 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 					if (!(ov || oh))
 						++st.xc_undecided;
 					else if (ov != occ_exact || (oh && occ_exact))
-						++st.xc_wrong;
+					{
+						if (++st.xc_wrong < 5)
+							print_case("exact_centre", d0, d1, b0, b1, occ_exact, ov);
+					}
 				}
 				// margins vs what they bound (only where the filter's domain conditions hold)
 				if (dbg.E == dbg.E && dbg.E < 1e30f && dbg.E > 0)
@@ -378,7 +422,7 @@ static void run(const Scenario& sc, uint64_t items, uint32_t seed, Stats& st)
 
 int main(int argc, char** argv)
 {
-	const Scenario scenarios[] = { { "c4", 0 }, { "biglocal", 1 }, { "hostile", 2 }, { "near", 3 }, { "farworld", 4 } };
+	const Scenario scenarios[] = { { "c4", 0 }, { "biglocal", 1 }, { "hostile", 2 }, { "near", 3 }, { "farworld", 4 }, { "subnormal", 5 } };
 	if (argc < 4)
 	{
 		fprintf(stderr, "usage: %s <scenario|all> <items> <seed> [threads]\n", argv[0]);

@@ -1,6 +1,7 @@
 """CPU-only checks of the conservative meshlet filter (niagara_b200/csrc/nvc_filter.cuh):
   * tests/filter_harness.cpp — millions of random / hostile meshlets through filter_meshlet (both Hi-Z access variants) against
-    the exact per-meshlet test, with the approximate reciprocals / roots perturbed by +-2 ulp: no decided item may disagree,
+    the exact per-meshlet test, with the approximate reciprocals / roots perturbed by +-2 ulp and flushed as the device's .ftz
+    instructions flush (the "subnormal" scenario puts znear, scale and view-space magnitudes there): no decided item may disagree,
     the margins must dominate the errors they bound, and the share of undecided items must stay small on the bench-like scene;
   * the filtered kernel (emulated) is exercised with the filter on / off and its diagnostic counters are read back."""
 import ctypes
@@ -35,10 +36,10 @@ def _harness():
 def test_filter_never_disagrees_with_the_exact_test(seed):
     res = subprocess.run([_harness(), "all", "3000000", str(seed), "4"], capture_output=True, text=True, timeout=600)
     lines = [json.loads(l) for l in res.stdout.splitlines() if l.startswith("{")]
-    assert len(lines) == 5, res.stderr[-2000:]
+    assert len(lines) == 6, res.stderr[-2000:]
     by = {l["scenario"]: l for l in lines}
     for name, l in by.items():
-        assert l["wrong"] == 0, (name, l)
+        assert l["wrong"] == 0, (name, l, res.stderr[-2000:])
         assert l["exact_centre_occlusion"]["wrong"] == 0 and l["exact_centre_occlusion"]["items"] > 100000, (name, l)  # the drawcull use
         assert l["max_center_err_over_E"] < 1.0 and l["max_uv_err_over_margin"] < 1.0, (name, l)
     assert res.returncode == 0
@@ -46,6 +47,10 @@ def test_filter_never_disagrees_with_the_exact_test(seed):
     assert by["c4"]["undecided"] < 0.08, by["c4"]
     assert by["biglocal"]["undecided"] < 0.08
     assert by["hostile"]["exact_only"] > 0.5
+    # the flush range: most cone tests there are left to the exact path (|c|^2 < 2^-110), but the filter still decides the rest
+    sub = by["subnormal"]
+    print("subnormal scenario: undecided %.4f (frustum / cone %.4f, domain %.4f), exact-centre occlusion undecided %.4f" % (sub["undecided"], sub["undecided_by_stage"]["frustum_cone"], sub["undecided_by_stage"]["domain"], sub["exact_centre_occlusion"]["undecided"]))
+    assert 0.05 < sub["undecided"] < 0.9 and sub["exact_centre_occlusion"]["undecided"] < 0.9, sub
 
 
 def test_filter_on_off_same_results_and_counters(golden_dir):
