@@ -787,6 +787,34 @@ NVC_API int nvc_cook_mesh_lods(NvcContext* ctx, void* stream, const NvcVertex* v
  * LODs of c0 = lods[0].indexCount and c(l+1) = the largest multiple of 3 below size_t(double(c(l)) * 0.85). */
 NVC_API int nvc_cook_mesh_lods_capacity(const NvcMesh* host_meshes, uint32_t mesh_count, uint32_t* indices_out);
 
+/* Turns what an importer produces into the processed Vertex[] and LOD 0 that nvc_cook_mesh_lods takes, bit-identical to the
+ * reference's cooker (scene.cpp:172-184 appendMesh: meshopt_filterIndexBuffer over the 6 position bytes,
+ * meshopt_generateVertexRemap over all 16 bytes and the remap of both buffers, meshopt_optimizeVertexCache,
+ * meshopt_optimizeVertexFetch):
+ *   vertices / vertex_count   device: Vertex[] as loadObj / loadVertices leave it (nvc_gltf_primitive_data's vertices)
+ *   indices / index_count     device: mesh-local indices
+ *   host_meshes / mesh_count  host: vertexOffset, vertexCount and lods[0].indexOffset / indexCount are read
+ *   meshes                    device out: vertexOffset / vertexCount of the mesh's vertices in vertices_out, lods[0] its range
+ *                             in lod0_out, lodCount 1, every other field 0; after a download, nvc_cook_mesh_lods' host_meshes
+ *   vertices_out              device out: the processed Vertex[], meshes in order; vertex_capacity >= vertex_count and >= the
+ *                             sum of the meshes' vertexCount
+ *   lod0_out                  device out: the mesh-local LOD 0 indices, meshes in order; index_capacity >= index_count and >=
+ *                             the sum of the meshes' lods[0].indexCount
+ *   totals4                   device out: vertices written, indices written, meshes rejected, 0
+ * A triangle is dropped when two corners have the same position bytes (so +-0 and NaN payloads stay distinct), or when an
+ * earlier kept triangle of the mesh is the same cyclic sequence of positions (a reversed triangle is not); kept triangles
+ * keep their order.  Vertices no kept triangle references are dropped.  A mesh with an index >= its vertexCount is
+ * rejected: it gets vertexCount 0 and an empty LOD 0, none of its vertices is read, and it is counted in totals4[2]; a mesh
+ * whose triangles are all dropped gets the same record.  NVC_ERROR_INVALID_ARGUMENT: an indexCount not a multiple of 3, an
+ * index or vertex range outside indices / vertices, or a capacity below the above; nothing is written then.
+ * NVC_ERROR_OUT_OF_MEMORY beyond 2^30 mesh vertices in one call.  Every step but the vertex cache optimisation (one
+ * sequential CTA per mesh) is data-parallel over all meshes.  Scratch is context-owned (about 24 bytes per index and 56 per
+ * vertex) and grows as needed, and the call synchronises the device before it enqueues its kernels on `stream`: call it at
+ * load time, outside stream capture. */
+NVC_API int nvc_cook_mesh_vertices(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices,
+    uint32_t index_count, const NvcMesh* host_meshes, uint32_t mesh_count, NvcMesh* meshes, NvcVertex* vertices_out, uint32_t vertex_capacity,
+    uint32_t* lod0_out, uint32_t index_capacity, uint32_t* totals4);
+
 #ifdef __cplusplus
 } /* extern "C" */
 

@@ -1053,3 +1053,126 @@ NVC_API int nvc_cook_mesh_lods(NvcContext* ctx, void* stream, const NvcVertex* v
 	e = nvc::launch_cook_mesh_lods(a, static_cast<cudaStream_t>(stream));
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_mesh_lods");
 }
+
+namespace
+{
+
+// The vertex cooker's walk over the meshes: per mesh its job (its first triangle and vertex slot, its vertex cache scratch
+// words), and the call's triangles, index positions, vertex slots and scratch words.
+struct VertexPlan
+{
+	std::vector<nvc::verts::VertexJob> jobs;
+	uint64_t triangles = 0, positions = 0, slots = 0, words = 0;
+	bool in_range = true; // every index and vertex range inside the call's buffers, index counts multiples of 3
+};
+
+VertexPlan plan_vertices(const NvcMesh* meshes, uint32_t mesh_count, uint64_t vertex_count, uint64_t index_count)
+{
+	VertexPlan plan;
+	plan.jobs.resize(mesh_count);
+	for (uint32_t i = 0; i < mesh_count; ++i)
+	{
+		const NvcMesh& mesh = meshes[i];
+		nvc::verts::VertexJob& job = plan.jobs[i];
+		job.vertex_offset = mesh.vertexOffset;
+		job.vertex_count = mesh.vertexCount;
+		job.index_offset = mesh.lods[0].indexOffset;
+		job.index_count = mesh.lods[0].indexCount;
+		job.tri_base = uint32_t(plan.triangles);
+		job.slot_base = uint32_t(plan.slots);
+		job.scratch = plan.words;
+		plan.words += nvc::vertex_cache_words(std::min(job.vertex_count, job.index_count), job.index_count);
+		plan.triangles += job.index_count / 3;
+		plan.positions += job.index_count;
+		plan.slots += job.vertex_count;
+		plan.in_range = plan.in_range && job.index_count % 3 == 0 && uint64_t(job.index_offset) + job.index_count <= index_count &&
+		                uint64_t(job.vertex_offset) + job.vertex_count <= vertex_count;
+	}
+	return plan;
+}
+
+} // namespace
+
+NVC_API int nvc_cook_mesh_vertices(NvcContext* ctx, void* stream, const NvcVertex* vertices, uint32_t vertex_count, const uint32_t* indices,
+    uint32_t index_count, const NvcMesh* host_meshes, uint32_t mesh_count, NvcMesh* meshes, NvcVertex* vertices_out, uint32_t vertex_capacity,
+    uint32_t* lod0_out, uint32_t index_capacity, uint32_t* totals4)
+{
+	if (!ctx || !totals4 || (mesh_count && (!host_meshes || !meshes)))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if ((vertex_count && !vertices) || (index_count && !indices) || (vertex_capacity && !vertices_out) || (index_capacity && !lod0_out))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	const VertexPlan plan = plan_vertices(host_meshes, mesh_count, vertex_count, index_count);
+	// neither output outgrows its input, counted per mesh (meshes may share ranges)
+	if (!plan.in_range || vertex_capacity < std::max<uint64_t>(vertex_count, plan.slots) || index_capacity < std::max<uint64_t>(index_count, plan.positions))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (plan.slots > (1u << 30))
+		return NVC_ERROR_OUT_OF_MEMORY; // the class table would need 2^32 buckets
+
+	const std::vector<nvc::verts::VertexJob>& jobs = plan.jobs;
+	std::vector<uint32_t> order(mesh_count);
+	for (uint32_t i = 0; i < mesh_count; ++i)
+		order[i] = i;
+	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+
+	const size_t M = mesh_count, T = plan.triangles, N = plan.positions, S = plan.slots;
+	const size_t tri_buckets = nvc::lods::hash_buckets(uint32_t(T)), vtx_buckets = nvc::lods::hash_buckets(uint32_t(S));
+	const size_t blocks = (N + nvc::verts::kScanItems - 1) / nvc::verts::kScanItems;
+	nvc::ScratchPlan sp;
+	const size_t o_jobs = sp.take(M * sizeof(nvc::verts::VertexJob)), o_order = sp.take(M * 4), o_rejected = sp.take(M);
+	const size_t o_ibase = sp.take(M * 4), o_vbase = sp.take(M * 4);
+	const size_t o_tri_table = sp.take(tri_buckets * 4), o_tri_entry = sp.take(T * 4);
+	const size_t o_flags = sp.take(N), o_rank = sp.take(N * 4), o_sums = sp.take(blocks * 4), o_offsets = sp.take((blocks + 1) * 8);
+	const size_t o_filtered = sp.take(N * 4), o_remapped = sp.take(N * 4);
+	const size_t o_first = sp.take(S * 4), o_vtx_table = sp.take(vtx_buckets * 4), o_vtx_first = sp.take(vtx_buckets * 4);
+	const size_t o_vtx_entry = sp.take(S * 4), o_classes = sp.take(S * 16), o_first_use = sp.take(S * 4), o_words = sp.take(plan.words * 4);
+
+	// the previous user of the scratch finishes first
+	cudaError_t e = cudaDeviceSynchronize();
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, "nvc_cook_mesh_vertices");
+	e = nvc::reserve_scratch(ctx, sp.bytes);
+	if (e != cudaSuccess)
+		return nvc::load_fail(ctx, e, "nvc_cook_mesh_vertices");
+	char* base = static_cast<char*>(ctx->load_scratch);
+	e = nvc::upload({ { base + o_jobs, jobs.data(), M * sizeof(nvc::verts::VertexJob) }, { base + o_order, order.data(), M * 4 } });
+	if (e != cudaSuccess)
+		return cuda_fail(ctx, e, "nvc_cook_mesh_vertices");
+
+	nvc::VertexArgs a;
+	a.vertices = vertices;
+	a.indices = indices;
+	a.jobs = reinterpret_cast<const nvc::verts::VertexJob*>(base + o_jobs);
+	a.order = reinterpret_cast<const uint32_t*>(base + o_order);
+	a.mesh_count = mesh_count;
+	a.tri_count = uint32_t(T);
+	a.position_count = uint32_t(N);
+	a.slot_count = uint32_t(S);
+	a.rejected = reinterpret_cast<uint8_t*>(base + o_rejected);
+	a.tri_table = reinterpret_cast<uint32_t*>(base + o_tri_table);
+	a.tri_mask = uint32_t(tri_buckets - 1);
+	a.tri_entry = reinterpret_cast<uint32_t*>(base + o_tri_entry);
+	a.flags = reinterpret_cast<uint8_t*>(base + o_flags);
+	a.rank = reinterpret_cast<uint32_t*>(base + o_rank);
+	a.block_sums = reinterpret_cast<uint32_t*>(base + o_sums);
+	a.offsets = reinterpret_cast<unsigned long long*>(base + o_offsets);
+	a.filtered = reinterpret_cast<uint32_t*>(base + o_filtered);
+	a.index_base = reinterpret_cast<uint32_t*>(base + o_ibase);
+	a.vertex_base = reinterpret_cast<uint32_t*>(base + o_vbase);
+	a.first = reinterpret_cast<uint32_t*>(base + o_first);
+	a.vtx_table = reinterpret_cast<uint32_t*>(base + o_vtx_table);
+	a.vtx_first = reinterpret_cast<uint32_t*>(base + o_vtx_first);
+	a.vtx_mask = uint32_t(vtx_buckets - 1);
+	a.vtx_entry = reinterpret_cast<uint32_t*>(base + o_vtx_entry);
+	a.classes = reinterpret_cast<NvcVertex*>(base + o_classes);
+	a.remapped = reinterpret_cast<uint32_t*>(base + o_remapped);
+	a.first_use = reinterpret_cast<uint32_t*>(base + o_first_use);
+	a.scratch = reinterpret_cast<uint32_t*>(base + o_words);
+	a.meshes = meshes;
+	a.vertices_out = vertices_out;
+	a.lod0_out = lod0_out;
+	a.totals4 = totals4;
+	e = nvc::launch_cook_mesh_vertices(a, static_cast<cudaStream_t>(stream));
+	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_mesh_vertices");
+}

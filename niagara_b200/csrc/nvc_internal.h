@@ -327,6 +327,55 @@ struct LodArgs
 	uint32_t* totals4;
 };
 cudaError_t launch_cook_mesh_lods(const LodArgs& a, cudaStream_t stream);
+namespace verts
+{
+// per mesh: its input ranges, its first triangle and first vertex slot among the call's, and its vertex cache scratch
+struct VertexJob
+{
+	uint32_t vertex_offset, vertex_count, index_offset, index_count;
+	uint32_t tri_base, slot_base;
+	uint64_t scratch;
+};
+constexpr uint32_t kScanItems = 2048; // flags per block of the scans
+}
+// nvc_cook_mesh_vertices (nvc_vertices.cuh): one job per mesh, in mesh order.  T = the call's triangles, N = 3 T its index
+// positions, S = the sum of the meshes' vertexCount (one slot per mesh vertex).  Every pointer is device memory.
+struct VertexArgs
+{
+	const NvcVertex* vertices;
+	const uint32_t* indices;
+	const verts::VertexJob* jobs;
+	const uint32_t* order; // mesh indices, longest LOD 0 first
+	uint32_t mesh_count;
+	uint32_t tri_count, position_count, slot_count; // T, N, S
+	uint8_t* rejected;             // per mesh
+	uint32_t* tri_table;           // hash_buckets(T): a triangle of each (mesh, rotated positions), the smallest
+	uint32_t tri_mask;
+	uint32_t* tri_entry;           // T: the triangle's bucket, or ~0 when it is dropped before the table
+	uint8_t* flags;                // N
+	uint32_t* rank;                // N: the last scan's result
+	uint32_t* block_sums;          // ceil(N / verts::kScanItems)
+	unsigned long long* offsets;   // that + 1
+	uint32_t* filtered;            // N: the kept triangles' indices, mesh-local
+	uint32_t* index_base;          // per mesh: its first filtered (= output) index
+	uint32_t* vertex_base;         // per mesh: its first class (= output vertex)
+	uint32_t* first;               // S: the first filtered position referencing the slot, ~0 when none
+	uint32_t* vtx_table;           // hash_buckets(S): a slot of each (mesh, 16 vertex bytes)
+	uint32_t* vtx_first;           // hash_buckets(S): the smallest `first` of the entry's class
+	uint32_t vtx_mask;
+	uint32_t* vtx_entry;           // S: the slot's bucket
+	NvcVertex* classes;            // S: the class vertices, in class order
+	uint32_t* remapped;            // N: the filtered indices remapped to classes
+	uint32_t* first_use;           // S: per class, its first position in the optimised indices
+	uint32_t* scratch;             // the jobs' vertex cache words
+	NvcMesh* meshes;
+	NvcVertex* vertices_out;
+	uint32_t* lod0_out;
+	uint32_t* totals4;
+};
+cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream);
+// the vertex cache scratch words of a mesh with at most `vertices` vertices and `indices` indices
+uint64_t vertex_cache_words(uint32_t vertices, uint32_t indices);
 // nvc_scene_cache_read_device (nvc_cache_decode.cuh).  Every pointer is device memory; `stream` is the section as stored,
 // padded so that word loads that cover its last byte stay inside the allocation.
 struct VertexDecodeArgs

@@ -16,6 +16,7 @@
 #include "nvc_filter.cuh"
 #include "nvc_cache_decode.cuh"
 #include "nvc_cache_encode.cuh"
+#include "nvc_vertices.cuh"
 
 #include <cuda_runtime.h>
 #include <string.h>
@@ -3453,6 +3454,91 @@ cudaError_t launch_cook_mesh_lods(const LodArgs& a, cudaStream_t stream)
 	if (a.mesh_count)
 		lods_copy_kernel<<<a.mesh_count, 256, 0, stream>>>(a);
 	return cudaGetLastError();
+}
+
+// ---- nvc_cook_mesh_vertices: appendMesh's vertex processing (nvc_vertices.cuh) ---------------------------------------------
+// exclusive scan of a.flags[0, n) into a.rank: block sums, their scan (one CTA), each block from its offset
+static void verts_scan(const VertexArgs& a, uint64_t n, cudaStream_t stream)
+{
+	using namespace verts;
+	const uint32_t blocks = uint32_t((n + verts::kScanItems - 1) / verts::kScanItems);
+	if (blocks)
+		verts_scan_reduce_kernel<<<blocks, verts::kThreads, 0, stream>>>(a.flags, n, a.block_sums);
+	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_sums, blocks, a.offsets);
+	if (blocks)
+		verts_scan_apply_kernel<<<blocks, verts::kThreads, 0, stream>>>(a.flags, n, a.offsets, a.rank);
+}
+
+uint64_t vertex_cache_words(uint32_t vertices, uint32_t indices)
+{
+	return verts::carve(vertices, indices, nullptr, nullptr);
+}
+
+cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream)
+{
+	using namespace verts;
+	const uint32_t T = a.tri_count, N = a.position_count, S = a.slot_count, M = a.mesh_count;
+	auto grid = [](uint32_t n) { return (n + verts::kThreads - 1) / verts::kThreads; };
+	cudaError_t e = cudaSuccess;
+	auto fill = [&](void* p, int value, size_t bytes) {
+		if (e == cudaSuccess && bytes)
+			e = cudaMemsetAsync(p, value, bytes, stream);
+	};
+	fill(a.totals4, 0, 16);
+	fill(a.rejected, 0, M);
+	fill(a.tri_table, 0xff, (size_t(a.tri_mask) + 1) * 4);
+	fill(a.vtx_table, 0xff, (size_t(a.vtx_mask) + 1) * 4);
+	fill(a.vtx_first, 0xff, (size_t(a.vtx_mask) + 1) * 4);
+	fill(a.first, 0xff, size_t(S) * 4);
+	fill(a.first_use, 0xff, size_t(S) * 4);
+	if (e != cudaSuccess)
+		return e;
+	// filter: rejection, then one thread per triangle, then the kept triangles compacted
+	if (T)
+	{
+		verts_reject_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
+		verts_filter_insert_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
+		verts_filter_flag_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
+	}
+	verts_scan(a, T, stream);
+	if (T)
+		verts_filter_compact_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
+	if (M)
+		verts_index_base_kernel<<<grid(M), verts::kThreads, 0, stream>>>(a);
+	// remap: first references, classes, their ranks over the filtered positions
+	fill(a.flags, 0, N);
+	if (N)
+		verts_first_kernel<<<grid(N), verts::kThreads, 0, stream>>>(a);
+	if (S)
+	{
+		verts_class_insert_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
+		verts_class_flag_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
+	}
+	verts_scan(a, N, stream);
+	if (M)
+		verts_mesh_kernel<<<grid(M), verts::kThreads, 0, stream>>>(a);
+	if (S)
+		verts_class_scatter_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
+	if (N)
+		verts_remap_kernel<<<grid(N), verts::kThreads, 0, stream>>>(a);
+	// vertex cache, one mesh per single-thread CTA
+	if (M)
+		verts_vcache_kernel<<<M, 1, 0, stream>>>(a);
+	// fetch order
+	fill(a.flags, 0, N);
+	if (e != cudaSuccess)
+		return e;
+	if (N)
+		verts_fetch_first_kernel<<<grid(N), verts::kThreads, 0, stream>>>(a);
+	if (S)
+		verts_fetch_flag_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
+	verts_scan(a, N, stream);
+	if (S)
+		verts_fetch_scatter_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
+	if (N)
+		verts_fetch_index_kernel<<<grid(N), verts::kThreads, 0, stream>>>(a);
+	return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 // N3: draws[update_indices[i]] = update_values[i]; one thread per 16-byte third of a 48-byte MeshDraw

@@ -110,6 +110,12 @@ SIGNATURES = [
         [c_void_p, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, c_void_p,
          ctypes.c_uint32, c_void_p],
     ),
+    (
+        "nvc_cook_mesh_vertices",
+        ctypes.c_int,
+        [c_void_p, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, c_void_p, ctypes.c_uint32,
+         c_void_p, ctypes.c_uint32, c_void_p],
+    ),
     ("nvc_nccl_unique_id", ctypes.c_int, [c_void_p]),
     ("nvc_nccl_init", ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int, ctypes.c_int]),
     ("nvc_allgather_visible", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_void_p]),
