@@ -815,6 +815,51 @@ NVC_API int nvc_cook_mesh_vertices(NvcContext* ctx, void* stream, const NvcVerte
     uint32_t index_count, const NvcMesh* host_meshes, uint32_t mesh_count, NvcMesh* meshes, NvcVertex* vertices_out, uint32_t vertex_capacity,
     uint32_t* lod0_out, uint32_t index_capacity, uint32_t* totals4);
 
+/* ---- OBJ import (loadMesh's loadObj, src/scene.cpp:117-168, over extern/fast_obj) --------------------------------------------- */
+typedef struct NvcObjFile
+{
+	const void* data; /* host: the file's bytes, as read from disk */
+	uint64_t size;
+} NvcObjFile;
+
+typedef struct NvcObjInfo
+{
+	uint64_t bytes_parsed;                                  /* where fast_obj's reader stops (the 64 KiB rule below) */
+	uint32_t position_count, texcoord_count, normal_count; /* v / vt / vn lines; the dummy element 0 is not counted */
+	uint32_t face_count;                                    /* faces pushed */
+	uint64_t index_count;                                   /* index records pushed, orphans included */
+	uint64_t corner_offset, corner_count;                   /* the file's range of `vertices`: the sum of 3 * (face_vertices - 2) */
+} NvcObjInfo;
+
+/* Loads OBJ files on the device: `vertices` gets, file after file, the Vertex[] the reference's loadObj returns for each, bit
+ * for bit (one 16-byte record per triangle corner: fp16 position, tp 0, three 10-bit snorm normal fields + 511, fp16 texcoord).
+ *   files / file_count   host: each file's bytes; they are uploaded into context-owned scratch
+ *   vertices             device out (16-byte aligned), or NULL to query: then only `infos` is written
+ *   vertex_capacity      records `vertices` holds; below the call's corners: NVC_ERROR_INVALID_ARGUMENT, `infos` still filled
+ *   infos                host out, file_count entries
+ * loadMesh gives appendMesh the identity indices, so file f is nvc_cook_mesh_vertices' mesh with vertexOffset = corner_offset,
+ * vertexCount = corner_count and lods[0] = { corner_offset, corner_count } over the indices 0..n-1.
+ * The file is parsed as fast_obj parses it: read in 64 KiB blocks of whole lines, a full block without '\n' ends the parse (a
+ * line of more than 64 KiB truncates the file there), a final line without '\n' is parsed.  `v` pushes 3 numbers, `vt` 2,
+ * `vn` 3, missing ones 0; `f` pushes one index record per `v`, `v/t`, `v//n` or `v/t/n`, negative indices relative to the
+ * counts at that line, and a vertex index of 0 (or anything that is not a number) ends the line without a face, the records
+ * before it staying in the index stream, which loadObj walks by the running sum of the face sizes.  Every other line is
+ * ignored; `mtllib` is not followed (materials cannot change loadObj's output, and there is no base path for file bytes).  A
+ * number is accumulated as fast_obj does in binary64; a NaN it produces is 0xffc00000, as on x86, the reference's platform.
+ * Refusals, decided before anything is written to `vertices`:
+ *   NVC_ERROR_CORRUPT       a face of fewer than 3 vertices, or a corner loadObj reads with a position, texcoord or normal
+ *                           index past the file's final count (the reference crashes or reads out of bounds on these);
+ *                           `infos` is filled, with such faces counted as 0 corners
+ *   NVC_ERROR_UNSUPPORTED   4 GiB or more of files in one call, 2^32 or more corners in one call, or a file whose arrays
+ *                           would overflow fast_obj's 32-bit sizes; `infos` is filled when the files were parsed
+ *   NVC_ERROR_INVALID_ARGUMENT  a NULL context or infos, a NULL file with bytes, a misaligned `vertices`, or the capacity above
+ * Index values of 10 or more digits wrap modulo 2^32, as the reference's x86 build does.  Scratch is context-owned (about
+ * 90 bytes per line, 12 per index record and 24 per face, plus the files); the call synchronises the device before it touches it, after
+ * the upload and before it reads back the counts and flags, and enqueues its kernels on `stream`: call it at load time,
+ * outside stream capture. */
+NVC_API int nvc_obj_load(NvcContext* ctx, void* stream, const NvcObjFile* files, uint32_t file_count, NvcVertex* vertices, uint64_t vertex_capacity,
+    NvcObjInfo* infos);
+
 #ifdef __cplusplus
 } /* extern "C" */
 

@@ -1176,3 +1176,194 @@ NVC_API int nvc_cook_mesh_vertices(NvcContext* ctx, void* stream, const NvcVerte
 	e = nvc::launch_cook_mesh_vertices(a, static_cast<cudaStream_t>(stream));
 	return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_cook_mesh_vertices");
 }
+
+namespace
+{
+
+// nvc_obj_load's scratch, in three parts, each planned once the counts it needs are known: the files and their line index;
+// the per-line arrays (L line slots); the parsed arrays (the call's v / vt / vn lines, index records and faces).
+struct ObjLayout
+{
+	size_t files, text, tile_lines, tile_offsets, part1;
+	size_t state, line_end, counts, block_sums, block_offsets, prefix, infos, part2;
+	size_t positions, texcoords, normals, records, faces, part3;
+};
+
+ObjLayout plan_obj(uint32_t file_count, uint64_t text_bytes, uint32_t tiles, uint64_t lines, const uint64_t* totals)
+{
+	using namespace nvc::obj;
+	const uint64_t F = file_count, blocks = (lines + kScanItems - 1) / kScanItems;
+	ObjLayout o;
+	nvc::ScratchPlan sp;
+	o.files = sp.take((F + 1) * sizeof(File));
+	o.text = sp.take(text_bytes);
+	o.tile_lines = sp.take(size_t(tiles) * 4);
+	o.tile_offsets = sp.take((size_t(tiles) + 1) * 8);
+	o.part1 = sp.bytes;
+	o.state = sp.take(F * sizeof(FileState));
+	o.line_end = sp.take(lines * 4);
+	o.counts = sp.take(kFields * lines * 4);
+	o.block_sums = sp.take(kFields * blocks * 4);
+	o.block_offsets = sp.take(kFields * (blocks + 1) * 8);
+	o.prefix = sp.take(kFields * (lines + 1) * 8);
+	o.infos = sp.take(F * sizeof(NvcObjInfo));
+	o.part2 = sp.bytes;
+	o.positions = sp.take((totals[kPositions] + F) * 12);
+	o.texcoords = sp.take((totals[kTexcoords] + F) * 8);
+	o.normals = sp.take((totals[kNormals] + F) * 12);
+	o.records = sp.take(totals[kRecords] * sizeof(Record));
+	o.faces = sp.take(totals[kFaces] * sizeof(Face));
+	o.part3 = sp.bytes;
+	return o;
+}
+
+// fast_obj's arrays hold 32-bit sizes, and growing one rounds its capacity up to 16 elements
+bool obj_arrays_fit(const NvcObjInfo& info)
+{
+	const uint64_t limit = 0xffffffffull - 15;
+	return 3 * (uint64_t(info.position_count) + 1) <= limit && 2 * (uint64_t(info.texcoord_count) + 1) <= limit &&
+	       3 * (uint64_t(info.normal_count) + 1) <= limit && info.index_count <= limit;
+}
+
+} // namespace
+
+NVC_API int nvc_obj_load(NvcContext* ctx, void* stream, const NvcObjFile* files, uint32_t file_count, NvcVertex* vertices, uint64_t vertex_capacity,
+    NvcObjInfo* infos)
+{
+	using namespace nvc::obj;
+	if (!ctx || (file_count && (!files || !infos)) || (reinterpret_cast<uintptr_t>(vertices) & 15))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	uint64_t size_sum = 0;
+	for (uint32_t f = 0; f < file_count; ++f)
+	{
+		if (files[f].size && !files[f].data)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		size_sum += std::min<uint64_t>(files[f].size, 1ull << 40);
+	}
+	if (!device_is_current(ctx))
+		return NVC_ERROR_INVALID_ARGUMENT;
+	if (file_count == 0)
+		return NVC_OK;
+	if (size_sum > 0xffffffffull)
+		return NVC_ERROR_UNSUPPORTED; // line ends, index records and window starts are 32-bit
+
+	std::vector<File> jobs(file_count + 1);
+	uint64_t text_bytes = 0, tiles = 0;
+	for (uint32_t f = 0; f < file_count; ++f)
+	{
+		jobs[f].data = text_bytes;
+		jobs[f].size = uint32_t(files[f].size);
+		jobs[f].tile_base = uint32_t(tiles);
+		text_bytes += (files[f].size + 15) & ~15ull;
+		tiles += (files[f].size + kTileBytes - 1) / kTileBytes;
+	}
+	jobs[file_count] = File{ text_bytes, 0, uint32_t(tiles) };
+
+	const cudaStream_t s = static_cast<cudaStream_t>(stream);
+	uint64_t lines = 0, totals[kFields] = {};
+	std::vector<NvcObjInfo> info(file_count);
+	std::vector<FileState> state(file_count);
+	// a part that does not fit the scratch grows it, and the call starts over from the upload (at most twice)
+	for (;;)
+	{
+		ObjLayout o = plan_obj(file_count, text_bytes, uint32_t(tiles), lines, totals);
+		// the previous user of the scratch finishes first
+		cudaError_t e = cudaDeviceSynchronize();
+		if (e == cudaSuccess)
+			e = nvc::reserve_scratch(ctx, o.part3); // the parts not planned yet are empty
+		if (e != cudaSuccess)
+			return nvc::load_fail(ctx, e, "nvc_obj_load");
+		char* base = static_cast<char*>(ctx->load_scratch);
+		nvc::ObjArgs a = {};
+		a.text = reinterpret_cast<const uint8_t*>(base + o.text);
+		a.files = reinterpret_cast<const File*>(base + o.files);
+		a.file_count = file_count;
+		a.tile_count = uint32_t(tiles);
+		a.tile_lines = reinterpret_cast<uint32_t*>(base + o.tile_lines);
+		a.tile_offsets = reinterpret_cast<unsigned long long*>(base + o.tile_offsets);
+		e = cudaMemcpy(base + o.files, jobs.data(), jobs.size() * sizeof(File), cudaMemcpyHostToDevice);
+		for (uint32_t f = 0; f < file_count && e == cudaSuccess; ++f)
+			if (files[f].size)
+				e = cudaMemcpy(base + o.text + jobs[f].data, files[f].data, files[f].size, cudaMemcpyHostToDevice);
+		// a copy from pageable memory is not ordered with a non-blocking stream
+		if (e == cudaSuccess)
+			e = cudaDeviceSynchronize();
+		if (e == cudaSuccess)
+			e = nvc::launch_obj_lines(a, s);
+		unsigned long long newlines = 0;
+		if (e == cudaSuccess)
+			e = cudaDeviceSynchronize();
+		if (e == cudaSuccess)
+			e = cudaMemcpy(&newlines, a.tile_offsets + tiles, 8, cudaMemcpyDeviceToHost);
+		if (e != cudaSuccess)
+			return cuda_fail(ctx, e, "nvc_obj_load");
+
+		// part 2: one line slot per '\n', and one per file for a last line without one
+		if (newlines + file_count > 0xffffffffull)
+			return NVC_ERROR_UNSUPPORTED;
+		lines = newlines + file_count;
+		o = plan_obj(file_count, text_bytes, uint32_t(tiles), lines, totals);
+		if (o.part2 > ctx->load_scratch_bytes)
+			continue;
+		a.line_slots = uint32_t(lines);
+		a.scan_blocks = uint32_t((lines + kScanItems - 1) / kScanItems);
+		a.line_end = reinterpret_cast<uint32_t*>(base + o.line_end);
+		a.state = reinterpret_cast<FileState*>(base + o.state);
+		a.counts = reinterpret_cast<uint32_t*>(base + o.counts);
+		a.block_sums = reinterpret_cast<uint32_t*>(base + o.block_sums);
+		a.block_offsets = reinterpret_cast<unsigned long long*>(base + o.block_offsets);
+		a.prefix = reinterpret_cast<unsigned long long*>(base + o.prefix);
+		a.infos = reinterpret_cast<NvcObjInfo*>(base + o.infos);
+		e = nvc::launch_obj_count(a, s);
+		if (e == cudaSuccess)
+			e = cudaDeviceSynchronize();
+		uint64_t now[kFields];
+		for (uint32_t k = 0; k < kFields && e == cudaSuccess; ++k)
+			e = cudaMemcpy(&now[k], a.prefix + uint64_t(k) * (lines + 1) + lines, 8, cudaMemcpyDeviceToHost);
+		if (e == cudaSuccess)
+			e = cudaMemcpy(info.data(), a.infos, file_count * sizeof(NvcObjInfo), cudaMemcpyDeviceToHost);
+		if (e == cudaSuccess)
+			e = cudaMemcpy(state.data(), a.state, file_count * sizeof(FileState), cudaMemcpyDeviceToHost);
+		if (e != cudaSuccess)
+			return cuda_fail(ctx, e, "nvc_obj_load");
+		memcpy(infos, info.data(), file_count * sizeof(NvcObjInfo));
+		bool fits = now[kCorners] <= 0xffffffffull;
+		for (uint32_t f = 0; f < file_count; ++f)
+			fits = fits && obj_arrays_fit(info[f]);
+		if (!fits)
+			return NVC_ERROR_UNSUPPORTED;
+		for (uint32_t f = 0; f < file_count; ++f)
+			if (state[f].flags & kBadFace)
+				return NVC_ERROR_CORRUPT;
+
+		// part 3: the parsed arrays
+		memcpy(totals, now, sizeof(now));
+		o = plan_obj(file_count, text_bytes, uint32_t(tiles), lines, totals);
+		if (o.part3 > ctx->load_scratch_bytes)
+			continue;
+		a.positions = reinterpret_cast<float*>(base + o.positions);
+		a.texcoords = reinterpret_cast<float*>(base + o.texcoords);
+		a.normals = reinterpret_cast<float*>(base + o.normals);
+		a.records = reinterpret_cast<Record*>(base + o.records);
+		a.faces = reinterpret_cast<Face*>(base + o.faces);
+		a.face_count = uint32_t(totals[kFaces]);
+		a.corner_count = totals[kCorners];
+		e = nvc::launch_obj_parse(a, s);
+		if (e == cudaSuccess)
+			e = cudaDeviceSynchronize();
+		if (e == cudaSuccess)
+			e = cudaMemcpy(state.data(), a.state, file_count * sizeof(FileState), cudaMemcpyDeviceToHost);
+		if (e != cudaSuccess)
+			return cuda_fail(ctx, e, "nvc_obj_load");
+		for (uint32_t f = 0; f < file_count; ++f)
+			if (state[f].flags & kBadIndex)
+				return NVC_ERROR_CORRUPT;
+		if (!vertices)
+			return NVC_OK;
+		if (vertex_capacity < a.corner_count)
+			return NVC_ERROR_INVALID_ARGUMENT;
+		a.vertices = vertices;
+		e = nvc::launch_obj_expand(a, s);
+		return e == cudaSuccess ? NVC_OK : cuda_fail(ctx, e, "nvc_obj_load");
+	}
+}

@@ -91,13 +91,14 @@ NVC_HD uint16_t quantize_half(float v)
 	return uint16_t(s | h);
 }
 
-// meshoptimizer.h:1133-1143 with N = 8
-NVC_HD int quantize_snorm8(float v)
+// meshoptimizer.h:1133-1143: N-bit snorm, N = 8 for cone axes and 10 for OBJ normals
+NVC_HD int quantize_snorm(float v, int N)
 {
+	const float scale = float((1 << (N - 1)) - 1);
 	float round = v >= 0 ? 0.5f : -0.5f;
 	v = v >= -1 ? v : -1;
 	v = v <= +1 ? v : +1;
-	return int(add(mul(v, 127.0f), round));
+	return int(add(mul(v, scale), round));
 }
 
 NVC_HD float dot3(const float* a, const V3& p) { return add(add(mul(a[0], p.x), mul(a[1], p.y)), mul(a[2], p.z)); }
@@ -310,7 +311,7 @@ NVC_HD void meshlet_bounds(const MeshletView& m, NvcMeshlet* out)
 			float err = cutoff;
 			for (int i = 0; i < 3; ++i)
 			{
-				int q = quantize_snorm8(axis[i]);
+				int q = quantize_snorm(axis[i], 8);
 				axis_s8[i] = int8_t(q);
 				err = add(err, fabsf(sub(div(float(int(axis_s8[i])), 127.0f), axis[i]))); // :264-269, summed left to right
 			}

@@ -376,6 +376,91 @@ struct VertexArgs
 cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream);
 // the vertex cache scratch words of a mesh with at most `vertices` vertices and `indices` indices
 uint64_t vertex_cache_words(uint32_t vertices, uint32_t indices);
+namespace obj
+{
+constexpr uint32_t kTileBytes = 4096;   // bytes per line-index tile: 256 threads x 16
+constexpr uint32_t kBlockBytes = 65536; // fast_obj's read block
+constexpr uint32_t kTilesPerBlock = kBlockBytes / kTileBytes;
+constexpr uint32_t kScanItems = 2048;   // lines per block of the count scans
+// the per-line counts, scanned into per-line prefixes over the call's lines
+enum Field : uint32_t
+{
+	kPositions,
+	kTexcoords,
+	kNormals,
+	kRecords,     // index records pushed, orphans included
+	kFaces,       // faces pushed
+	kFaceIndices, // a face's vertex count, 0 for other lines: the running sum locates loadObj's windows
+	kCorners,     // 3 * (vertices - 2) for a face of 3 or more vertices
+	kFields
+};
+constexpr uint32_t kBadFace = 1;  // a face of fewer than 3 vertices
+constexpr uint32_t kBadIndex = 2; // a corner loadObj reads has an index past the file's final count
+// per file, host-built, plus a sentinel whose tile_base is the call's tile count
+struct File
+{
+	uint64_t data;      // its first byte in ObjArgs::text (16-byte aligned)
+	uint32_t size;
+	uint32_t tile_base; // its first tile among the call's
+};
+// per file, device-computed
+struct FileState
+{
+	uint32_t cut;        // the first full 64 KiB block without '\n' (the reader stops there), ~0 when none
+	uint32_t first_line; // its first line slot: the '\n' bytes of the files before it + its index
+	uint32_t line_count; // the lines the reader parses
+	uint32_t flags;      // kBadFace | kBadIndex
+	uint32_t positions, texcoords, normals; // final counts (v, vt and vn lines parsed)
+	uint32_t pad;
+	uint64_t position_base, texcoord_base, normal_base; // its element 0 (the dummy) in the call's arrays
+};
+struct Record
+{
+	uint32_t p, t, n; // resolved as fast_obj resolves them, file-local
+};
+struct Face
+{
+	uint32_t window; // its first index record: the file's first record + the face vertices of the file's earlier faces
+	uint32_t count;
+	uint32_t file, pad;
+	uint64_t corner; // its first output record
+};
+}
+// nvc_obj_load (nvc_obj.cuh).  L = the call's line slots: its '\n' bytes plus one per file (a final line without '\n').
+// Every pointer is device memory.
+struct ObjArgs
+{
+	const uint8_t* text;
+	const obj::File* files; // file_count + 1
+	uint32_t file_count, tile_count;
+	uint32_t* tile_lines;                 // per tile: its '\n' bytes
+	unsigned long long* tile_offsets;     // tile_count + 1: their exclusive scan
+	uint32_t line_slots;                  // L
+	uint32_t scan_blocks;                 // ceil(L / obj::kScanItems)
+	uint32_t* line_end;                   // L: the line's '\n' (or the file's end), file-relative
+	obj::FileState* state;                // file_count
+	uint32_t* counts;                     // kFields x L
+	uint32_t* block_sums;                 // kFields x scan_blocks
+	unsigned long long* block_offsets;    // kFields x (scan_blocks + 1)
+	unsigned long long* prefix;           // kFields x (L + 1): exclusive scans of `counts`, the totals last
+	float* positions;                     // 3 per element, each file's dummy first
+	float* texcoords;                     // 2 per element
+	float* normals;                       // 3 per element
+	obj::Record* records;                 // the index stream
+	obj::Face* faces;                     // the face list
+	uint32_t face_count;
+	uint64_t corner_count;
+	NvcObjInfo* infos;                    // file_count
+	NvcVertex* vertices;
+};
+// line index: the tiles' '\n' counts and their scan
+cudaError_t launch_obj_lines(const ObjArgs& a, cudaStream_t stream);
+// line ends, the reader's cut, per-line counts and their scans, per-file infos
+cudaError_t launch_obj_count(const ObjArgs& a, cudaStream_t stream);
+// numbers, index records, faces, the range check
+cudaError_t launch_obj_parse(const ObjArgs& a, cudaStream_t stream);
+// the Vertex[] records
+cudaError_t launch_obj_expand(const ObjArgs& a, cudaStream_t stream);
 // nvc_scene_cache_read_device (nvc_cache_decode.cuh).  Every pointer is device memory; `stream` is the section as stored,
 // padded so that word loads that cover its last byte stay inside the allocation.
 struct VertexDecodeArgs

@@ -17,6 +17,7 @@
 #include "nvc_cache_decode.cuh"
 #include "nvc_cache_encode.cuh"
 #include "nvc_vertices.cuh"
+#include "nvc_obj.cuh"
 
 #include <cuda_runtime.h>
 #include <string.h>
@@ -3539,6 +3540,62 @@ cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream)
 	if (N)
 		verts_fetch_index_kernel<<<grid(N), verts::kThreads, 0, stream>>>(a);
 	return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+// ---- nvc_obj_load: loadObj over fast_obj (nvc_obj.cuh) -----------------------------------------------------------------------
+static uint32_t obj_grid(uint64_t n)
+{
+	return uint32_t((n + obj::kThreads - 1) / obj::kThreads);
+}
+
+cudaError_t launch_obj_lines(const ObjArgs& a, cudaStream_t stream)
+{
+	using namespace obj;
+	if (a.tile_count)
+		obj_tile_count_kernel<<<a.tile_count, obj::kThreads, 0, stream>>>(a);
+	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.tile_lines, a.tile_count, a.tile_offsets);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_obj_count(const ObjArgs& a, cudaStream_t stream)
+{
+	using namespace obj;
+	cudaError_t e = cudaMemsetAsync(a.state, 0xff, size_t(a.file_count) * sizeof(FileState), stream);
+	if (e != cudaSuccess)
+		return e;
+	if (a.tile_count)
+	{
+		obj_line_end_kernel<<<a.tile_count, obj::kThreads, 0, stream>>>(a);
+		obj_cut_kernel<<<obj_grid(a.tile_count), obj::kThreads, 0, stream>>>(a);
+	}
+	obj_file_kernel<<<obj_grid(a.file_count), obj::kThreads, 0, stream>>>(a);
+	obj_classify_kernel<<<obj_grid(a.line_slots), obj::kThreads, 0, stream>>>(a);
+	obj_scan_reduce_kernel<<<dim3(a.scan_blocks, kFields), obj::kThreads, 0, stream>>>(a);
+	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	for (uint32_t k = 0; k < kFields; ++k)
+		scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_sums + size_t(k) * a.scan_blocks, a.scan_blocks, a.block_offsets + size_t(k) * (a.scan_blocks + 1));
+	obj_scan_apply_kernel<<<dim3(a.scan_blocks, kFields), obj::kThreads, 0, stream>>>(a);
+	obj_info_kernel<<<obj_grid(a.file_count), obj::kThreads, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_obj_parse(const ObjArgs& a, cudaStream_t stream)
+{
+	using namespace obj;
+	obj_dummy_kernel<<<obj_grid(a.file_count), obj::kThreads, 0, stream>>>(a);
+	obj_parse_kernel<<<obj_grid(a.line_slots), obj::kThreads, 0, stream>>>(a);
+	if (a.face_count)
+		obj_check_kernel<<<obj_grid(a.face_count), obj::kThreads, 0, stream>>>(a);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_obj_expand(const ObjArgs& a, cudaStream_t stream)
+{
+	using namespace obj;
+	if (a.corner_count)
+		obj_expand_kernel<<<obj_grid(a.corner_count), obj::kThreads, 0, stream>>>(a);
+	return cudaGetLastError();
 }
 
 // N3: draws[update_indices[i]] = update_values[i]; one thread per 16-byte third of a 48-byte MeshDraw

@@ -116,6 +116,7 @@ SIGNATURES = [
         [c_void_p, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint32, c_void_p, c_void_p, ctypes.c_uint32,
          c_void_p, ctypes.c_uint32, c_void_p],
     ),
+    ("nvc_obj_load", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_uint32, c_void_p, ctypes.c_uint64, c_void_p]),
     ("nvc_nccl_unique_id", ctypes.c_int, [c_void_p]),
     ("nvc_nccl_init", ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int, ctypes.c_int]),
     ("nvc_allgather_visible", ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_void_p]),
