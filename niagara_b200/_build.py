@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libniagara_cull.so")
 
 SOURCES = ["nvc_kernels.cu", "nvc_api.cu", "nvc_peer.cu", "nvc_host.cpp", "nvc_scene_cache.cpp", "nvc_scene_cache_device.cpp", "nvc_scene_cache_write.cpp", "nvc_meshopt_decode.cpp", "nvc_meshopt_encode.cpp", "nvc_gltf.cpp", "nvc_nccl.cpp"]
-HEADERS = ["nvc_internal.h", "nvc_math.cuh", "nvc_filter.cuh", "nvc_cook.cuh", "nvc_meshlets.cuh", "nvc_lods.cuh", "nvc_vertices.cuh", "nvc_obj.cuh", "nvc_cache_decode.cuh", "nvc_cache_encode.cuh", "nvc_meshopt_format.h", "nvc_meshopt_host.h", "nvc_tma.cuh", os.path.join(ROOT, "include", "niagara_cull.h")]
+HEADERS = ["nvc_internal.h", "nvc_math.cuh", "nvc_filter.cuh", "nvc_cook.cuh", "nvc_meshlets.cuh", "nvc_lods.cuh", "nvc_vertices.cuh", "nvc_obj.cuh", "nvc_scan.cuh", "nvc_cache_decode.cuh", "nvc_cache_encode.cuh", "nvc_meshopt_format.h", "nvc_meshopt_host.h", "nvc_tma.cuh", os.path.join(ROOT, "include", "niagara_cull.h")]
 
 NVCC_FLAGS = [
     "-gencode",

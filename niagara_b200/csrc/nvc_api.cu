@@ -5,6 +5,7 @@
 #include "nvc_lods.cuh"
 
 #include <algorithm>
+#include <numeric>
 #include <vector>
 
 #include <stdio.h>
@@ -750,6 +751,15 @@ NVC_API int nvc_cook_meshlet_bounds(NvcContext* ctx, void* stream, const NvcVert
 namespace
 {
 
+// Sorts the job indices in [first, last) longest job (most indices) first, ties in index order: the cook kernels take jobs
+// in this order, so the longest sequential jobs start first.  Outputs are placed by job index, so the order does not
+// change them.
+template <typename It, typename Job>
+static void longest_first(It first, It last, const std::vector<Job>& jobs)
+{
+	std::stable_sort(first, last, [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+}
+
 // The meshlet cooker's walk over meshes x LODs, in mesh then LOD order: per LOD its job (the scratch ranges of
 // nvc_cook_meshlets laid out in that order) and whether it is the mesh's lodRT, and the sums of the per-LOD bounds.  The
 // capacity queries return the sums and the cook plans its call with the jobs, so that a capacity is what the call plans.
@@ -841,15 +851,12 @@ static int cook_meshlets(NvcContext* ctx, void* stream, const NvcVertex* vertice
 			rt_meshes.push_back(host_meshes[i]);
 			rt_meshes[i].lodRT = plan.mesh_rt[i];
 		}
-	// the longest jobs start first; outputs are placed by job index, so the order does not change them.  clrt: the greedy
-	// jobs, then the ray-tracing jobs, each longest first
+	// clrt: the greedy jobs, then the ray-tracing jobs, each longest first
 	std::vector<uint32_t> order(job_count);
-	for (uint32_t j = 0; j < job_count; ++j)
-		order[j] = j;
-	auto longer = [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; };
+	std::iota(order.begin(), order.end(), 0u);
 	auto rt_end = std::stable_partition(order.begin(), order.end(), [&](uint32_t x) { return !plan.job_rt[x]; });
-	std::stable_sort(order.begin(), rt_end, longer);
-	std::stable_sort(rt_end, order.end(), longer);
+	longest_first(order.begin(), rt_end, jobs);
+	longest_first(rt_end, order.end(), jobs);
 	const uint32_t greedy_count = uint32_t(rt_end - order.begin());
 
 	nvc::ScratchPlan sp;
@@ -1014,9 +1021,8 @@ NVC_API int nvc_cook_mesh_lods(NvcContext* ctx, void* stream, const NvcVertex* v
 	if (max_scale)
 		scales.assign(max_scale, max_scale + mesh_count);
 	std::vector<uint32_t> order(mesh_count);
-	for (uint32_t i = 0; i < mesh_count; ++i)
-		order[i] = i;
-	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+	std::iota(order.begin(), order.end(), 0u);
+	longest_first(order.begin(), order.end(), jobs);
 
 	const size_t n = mesh_count;
 	nvc::ScratchPlan sp;
@@ -1112,18 +1118,17 @@ NVC_API int nvc_cook_mesh_vertices(NvcContext* ctx, void* stream, const NvcVerte
 
 	const std::vector<nvc::verts::VertexJob>& jobs = plan.jobs;
 	std::vector<uint32_t> order(mesh_count);
-	for (uint32_t i = 0; i < mesh_count; ++i)
-		order[i] = i;
-	std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return jobs[x].index_count > jobs[y].index_count; });
+	std::iota(order.begin(), order.end(), 0u);
+	longest_first(order.begin(), order.end(), jobs);
 
 	const size_t M = mesh_count, T = plan.triangles, N = plan.positions, S = plan.slots;
 	const size_t tri_buckets = nvc::lods::hash_buckets(uint32_t(T)), vtx_buckets = nvc::lods::hash_buckets(uint32_t(S));
-	const size_t blocks = (N + nvc::verts::kScanItems - 1) / nvc::verts::kScanItems;
+	const size_t blocks = (N + nvc::scan::kScanItems - 1) / nvc::scan::kScanItems;
 	nvc::ScratchPlan sp;
 	const size_t o_jobs = sp.take(M * sizeof(nvc::verts::VertexJob)), o_order = sp.take(M * 4), o_rejected = sp.take(M);
 	const size_t o_ibase = sp.take(M * 4), o_vbase = sp.take(M * 4);
 	const size_t o_tri_table = sp.take(tri_buckets * 4), o_tri_entry = sp.take(T * 4);
-	const size_t o_flags = sp.take(N), o_rank = sp.take(N * 4), o_sums = sp.take(blocks * 4), o_offsets = sp.take((blocks + 1) * 8);
+	const size_t o_flags = sp.take(N), o_rank = sp.take((N + 1) * 4), o_sums = sp.take(blocks * 4), o_offsets = sp.take((blocks + 1) * 8);
 	const size_t o_filtered = sp.take(N * 4), o_remapped = sp.take(N * 4);
 	const size_t o_first = sp.take(S * 4), o_vtx_table = sp.take(vtx_buckets * 4), o_vtx_first = sp.take(vtx_buckets * 4);
 	const size_t o_vtx_entry = sp.take(S * 4), o_classes = sp.take(S * 16), o_first_use = sp.take(S * 4), o_words = sp.take(plan.words * 4);
@@ -1192,7 +1197,7 @@ struct ObjLayout
 ObjLayout plan_obj(uint32_t file_count, uint64_t text_bytes, uint32_t tiles, uint64_t lines, const uint64_t* totals)
 {
 	using namespace nvc::obj;
-	const uint64_t F = file_count, blocks = (lines + kScanItems - 1) / kScanItems;
+	const uint64_t F = file_count, blocks = (lines + nvc::scan::kScanItems - 1) / nvc::scan::kScanItems;
 	ObjLayout o;
 	nvc::ScratchPlan sp;
 	o.files = sp.take((F + 1) * sizeof(File));
@@ -1306,7 +1311,6 @@ NVC_API int nvc_obj_load(NvcContext* ctx, void* stream, const NvcObjFile* files,
 		if (o.part2 > ctx->load_scratch_bytes)
 			continue;
 		a.line_slots = uint32_t(lines);
-		a.scan_blocks = uint32_t((lines + kScanItems - 1) / kScanItems);
 		a.line_end = reinterpret_cast<uint32_t*>(base + o.line_end);
 		a.state = reinterpret_cast<FileState*>(base + o.state);
 		a.counts = reinterpret_cast<uint32_t*>(base + o.counts);

@@ -23,6 +23,7 @@
 
 #include "nvc_internal.h"
 #include "nvc_meshopt_format.h"
+#include "nvc_scan.cuh"
 
 namespace nvc
 {
@@ -54,6 +55,13 @@ __device__ __forceinline__ uint32_t column_value(const uint32_t (&v)[4], uint32_
 	return k == 0 ? v[0] : k == 1 ? v[1] : k == 2 ? v[2] : v[3];
 }
 
+// vcodec::combine of one column's channel, as a scan operation
+struct Combine
+{
+	uint32_t channel;
+	__device__ __forceinline__ uint32_t operator()(uint32_t x, uint32_t y) const { return vcodec::combine(x, y, channel); }
+};
+
 __device__ __forceinline__ uint32_t padded_word(uint32_t vertex, uint32_t column, uint32_t columns)
 {
 	return vertex * columns + column + vertex / 8u;
@@ -63,7 +71,6 @@ template <uint32_t S>
 __global__ void __launch_bounds__(kVertexWarps * 32) decode_vertex_blocks_kernel(const VertexDecodeArgs a)
 {
 	constexpr uint32_t C = S / 4;
-	const uint32_t full = 0xffffffffu;
 	__shared__ uint32_t s_stage[kVertexWarps][VertexStage<S>::words];
 	__shared__ __align__(8) uint8_t s_planes[kVertexWarps][S * kVertexBlock];
 	__shared__ uint16_t s_group[kVertexWarps][S * 16];
@@ -150,16 +157,7 @@ __global__ void __launch_bounds__(kVertexWarps * 32) decode_vertex_blocks_kernel
 			acc = vcodec::combine(acc, vcodec::delta_term(bytes4, channel), channel);
 			v[t] = acc;
 		}
-		uint32_t x = acc;
-		for (uint32_t d = 1; d < 32; d <<= 1)
-		{
-			uint32_t y = __shfl_up_sync(full, x, d);
-			if (lane >= d)
-				x = vcodec::combine(y, x, channel);
-		}
-		uint32_t before = __shfl_up_sync(full, x, 1);
-		if (lane == 0)
-			before = 0;
+		const uint32_t before = scan::warp_exclusive(acc, lane, Combine{ channel });
 		for (uint32_t t = 0; t < 8; ++t)
 		{
 			const uint32_t i = lane * 8 + t;
@@ -179,46 +177,12 @@ __global__ void __launch_bounds__(kVertexWarps * 32) decode_vertex_blocks_kernel
 template <uint32_t C>
 __global__ void __launch_bounds__(kCarryThreads) decode_vertex_carry_kernel(const VertexDecodeArgs a)
 {
-	const uint32_t full = 0xffffffffu;
 	__shared__ uint32_t s_warp[kCarryThreads / 32];
-	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
 	const uint32_t k = blockIdx.x, channel = column_value(a.channel, k);
-	uint32_t running = column_value(a.baseline, k);
-	for (uint32_t base = 0; base < a.blocks; base += kCarryThreads)
-	{
-		const uint32_t b = base + threadIdx.x;
-		uint32_t x = b < a.blocks ? a.carry[size_t(b) * C + k] : 0u;
-		for (uint32_t d = 1; d < 32; d <<= 1)
-		{
-			uint32_t y = __shfl_up_sync(full, x, d);
-			if (lane >= d)
-				x = vcodec::combine(y, x, channel);
-		}
-		if (lane == 31)
-			s_warp[warp] = x;
-		__syncthreads();
-		if (warp == 0)
-		{
-			uint32_t w = s_warp[lane];
-			for (uint32_t d = 1; d < 32; d <<= 1)
-			{
-				uint32_t y = __shfl_up_sync(full, w, d);
-				if (lane >= d)
-					w = vcodec::combine(y, w, channel);
-			}
-			s_warp[lane] = w;
-		}
-		__syncthreads();
-		uint32_t before = __shfl_up_sync(full, x, 1);
-		if (lane == 0)
-			before = warp ? s_warp[warp - 1] : 0u;
-		else if (warp)
-			before = vcodec::combine(s_warp[warp - 1], before, channel);
-		if (b < a.blocks)
-			a.carry[size_t(b) * C + k] = vcodec::combine(running, before, channel);
-		running = vcodec::combine(running, s_warp[kCarryThreads / 32 - 1], channel);
-		__syncthreads();
-	}
+	uint32_t* carry = a.carry + k;
+	scan::scan_tiles<kCarryThreads>(
+	    a.blocks, column_value(a.baseline, k), s_warp, [&](uint32_t b) { return carry[size_t(b) * C]; }, [&](uint32_t b, uint32_t v) { carry[size_t(b) * C] = v; },
+	    Combine{ channel });
 }
 
 template <uint32_t C>

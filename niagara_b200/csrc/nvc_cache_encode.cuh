@@ -13,8 +13,8 @@
 //             plane's control (all zero: 2; else the cheaper of the {0,1,2,4} / {1,2,4,8} width tables, unless neither beats
 //             `count` literal bytes: 3) and per group of 16 the width (the smallest size, scanning the table's last entry
 //             first; an equal size switches to the width the previous group used, never away from literals).  Run twice:
-//             the measure pass stores each block's size; after an exclusive scan the write pass stores the block where it
-//             belongs, control bytes first, then the planes in order.  The write pass also stores the header byte and the
+//             the measure pass stores each block's size; after their scan (scan::offsets_kernel) the write pass stores the
+//             block where it belongs, control bytes first, then the planes in order.  The write pass also stores the header byte and the
 //             tail (zeros up to 24 bytes, vertex 0, the channel bytes).
 // Meshlet codec.  One thread per meshlet, measure then write as above; a meshlet's record is its uint16 size, then the block
 // mcodec::decode_block reads back: the reference deltas, the explicit triangle bytes, the zero gap, the reference control
@@ -25,6 +25,7 @@
 
 #include "nvc_internal.h"
 #include "nvc_meshopt_format.h"
+#include "nvc_scan.cuh"
 
 namespace nvc
 {
@@ -33,7 +34,6 @@ namespace cache
 
 constexpr uint32_t kEncodeWarps = 4;
 constexpr uint32_t kEstimateThreads = 256;
-constexpr uint32_t kEncodeScanThreads = 1024;
 constexpr uint32_t kMeshletEncodeThreads = 128;
 
 // The delta byte of plane q for a vertex whose words are `cur`, after the vertex whose words are `prev` (C words each):
@@ -227,13 +227,7 @@ __global__ void __launch_bounds__(kEncodeWarps * 32) encode_vertex_blocks_kernel
 	}
 
 	// the planes' offsets in the block, after its control bytes
-	uint32_t at = size;
-	for (uint32_t d = 1; d < 32; d <<= 1)
-	{
-		const uint32_t y = __shfl_up_sync(full, at, d);
-		if (lane >= d)
-			at += y;
-	}
+	uint32_t at = scan::warp_inclusive(size, lane);
 	const uint32_t total = __shfl_sync(full, at, 31) + C;
 	at = at - size + C;
 	// the control byte of column `lane`: 2 bits per plane, from lanes 4 lane .. 4 lane + 3
@@ -291,50 +285,6 @@ __global__ void __launch_bounds__(kEncodeWarps * 32) encode_vertex_blocks_kernel
 			if (grp.byte(i) >= sentinel)
 				*p++ = uint8_t(grp.byte(i));
 	}
-}
-
-// ---- exclusive scan of per-item sizes into 64-bit offsets (offsets[n] = the total); one CTA --------------------------------
-// Each pass's sizes add up to less than 2^32 (an item is at most a few KB), so the passes scan 32-bit values.
-__global__ void __launch_bounds__(kEncodeScanThreads) encode_scan_kernel(const uint32_t* sizes, uint32_t n, unsigned long long* offsets)
-{
-	const uint32_t full = 0xffffffffu;
-	__shared__ uint32_t s_warp[kEncodeScanThreads / 32];
-	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-	unsigned long long running = 0;
-	for (uint32_t base = 0; base < n; base += kEncodeScanThreads)
-	{
-		const uint32_t i = base + threadIdx.x;
-		const uint32_t v = i < n ? sizes[i] : 0u;
-		uint32_t x = v;
-		for (uint32_t d = 1; d < 32; d <<= 1)
-		{
-			const uint32_t y = __shfl_up_sync(full, x, d);
-			if (lane >= d)
-				x += y;
-		}
-		if (lane == 31)
-			s_warp[warp] = x;
-		__syncthreads();
-		if (warp == 0)
-		{
-			uint32_t w = s_warp[lane];
-			for (uint32_t d = 1; d < 32; d <<= 1)
-			{
-				const uint32_t y = __shfl_up_sync(full, w, d);
-				if (lane >= d)
-					w += y;
-			}
-			s_warp[lane] = w;
-		}
-		__syncthreads();
-		const uint32_t before = x - v + (warp ? s_warp[warp - 1] : 0u);
-		if (i < n)
-			offsets[i] = running + before;
-		running += s_warp[kEncodeScanThreads / 32 - 1];
-		__syncthreads();
-	}
-	if (threadIdx.x == 0)
-		offsets[n] = running;
 }
 
 // ---- meshlet codec --------------------------------------------------------------------------------------------------------

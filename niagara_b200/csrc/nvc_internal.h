@@ -327,6 +327,10 @@ struct LodArgs
 	uint32_t* totals4;
 };
 cudaError_t launch_cook_mesh_lods(const LodArgs& a, cudaStream_t stream);
+namespace scan
+{
+constexpr uint32_t kScanItems = 2048; // values per block of nvc_scan.cuh's device-wide scan
+}
 namespace verts
 {
 // per mesh: its input ranges, its first triangle and first vertex slot among the call's, and its vertex cache scratch
@@ -336,7 +340,6 @@ struct VertexJob
 	uint32_t tri_base, slot_base;
 	uint64_t scratch;
 };
-constexpr uint32_t kScanItems = 2048; // flags per block of the scans
 }
 // nvc_cook_mesh_vertices (nvc_vertices.cuh): one job per mesh, in mesh order.  T = the call's triangles, N = 3 T its index
 // positions, S = the sum of the meshes' vertexCount (one slot per mesh vertex).  Every pointer is device memory.
@@ -353,8 +356,8 @@ struct VertexArgs
 	uint32_t tri_mask;
 	uint32_t* tri_entry;           // T: the triangle's bucket, or ~0 when it is dropped before the table
 	uint8_t* flags;                // N
-	uint32_t* rank;                // N: the last scan's result
-	uint32_t* block_sums;          // ceil(N / verts::kScanItems)
+	uint32_t* rank;                // N + 1: the last scan's result, its total last
+	uint32_t* block_sums;          // ceil(N / scan::kScanItems)
 	unsigned long long* offsets;   // that + 1
 	uint32_t* filtered;            // N: the kept triangles' indices, mesh-local
 	uint32_t* index_base;          // per mesh: its first filtered (= output) index
@@ -381,7 +384,6 @@ namespace obj
 constexpr uint32_t kTileBytes = 4096;   // bytes per line-index tile: 256 threads x 16
 constexpr uint32_t kBlockBytes = 65536; // fast_obj's read block
 constexpr uint32_t kTilesPerBlock = kBlockBytes / kTileBytes;
-constexpr uint32_t kScanItems = 2048;   // lines per block of the count scans
 // the per-line counts, scanned into per-line prefixes over the call's lines
 enum Field : uint32_t
 {
@@ -436,12 +438,11 @@ struct ObjArgs
 	uint32_t* tile_lines;                 // per tile: its '\n' bytes
 	unsigned long long* tile_offsets;     // tile_count + 1: their exclusive scan
 	uint32_t line_slots;                  // L
-	uint32_t scan_blocks;                 // ceil(L / obj::kScanItems)
 	uint32_t* line_end;                   // L: the line's '\n' (or the file's end), file-relative
 	obj::FileState* state;                // file_count
 	uint32_t* counts;                     // kFields x L
-	uint32_t* block_sums;                 // kFields x scan_blocks
-	unsigned long long* block_offsets;    // kFields x (scan_blocks + 1)
+	uint32_t* block_sums;                 // kFields x ceil(L / scan::kScanItems)
+	unsigned long long* block_offsets;    // kFields x (ceil(L / scan::kScanItems) + 1)
 	unsigned long long* prefix;           // kFields x (L + 1): exclusive scans of `counts`, the totals last
 	float* positions;                     // 3 per element, each file's dummy first
 	float* texcoords;                     // 2 per element

@@ -18,6 +18,7 @@
 #include "nvc_cache_encode.cuh"
 #include "nvc_vertices.cuh"
 #include "nvc_obj.cuh"
+#include "nvc_scan.cuh"
 
 #include <cuda_runtime.h>
 #include <string.h>
@@ -2371,16 +2372,6 @@ namespace
 constexpr uint32_t kCookWarps = 4;        // jobs per block of the build kernel
 constexpr uint32_t kCookScanThreads = 256; // the one block of the scan kernel
 
-__device__ __forceinline__ uint32_t cook_warp_inclusive(uint32_t v, uint32_t lane)
-{
-	for (uint32_t d = 1; d < 32; d <<= 1)
-	{
-		uint32_t o = __shfl_up_sync(0xffffffffu, v, d);
-		v += lane >= d ? o : 0u;
-	}
-	return v;
-}
-
 // Orders scores as floats do, with -0 == +0 and NaN above everything
 __device__ __forceinline__ uint32_t cook_score_key(float s)
 {
@@ -2410,8 +2401,8 @@ __device__ uint32_t cook_neighbor(uint32_t lane, const cook::Building& m, const 
 		v1 = mlv[m.vertex_offset + lane + 32];
 		c1 = counts[v1];
 	}
-	uint32_t p0 = cook_warp_inclusive(c0, lane);
-	uint32_t p1 = cook_warp_inclusive(c1, lane) + __shfl_sync(full, p0, 31);
+	uint32_t p0 = scan::warp_inclusive(c0, lane);
+	uint32_t p1 = scan::warp_inclusive(c1, lane) + __shfl_sync(full, p0, 31);
 	if (lane == 0)
 		s_prefix[0] = 0;
 	s_prefix[lane + 1] = p0;
@@ -2425,15 +2416,7 @@ __device__ uint32_t cook_neighbor(uint32_t lane, const cook::Building& m, const 
 	uint32_t bp = 5, bs = 0, bk = 0, bt = cook::kNone; // least (priority, score, k)
 	for (uint32_t k = lane; k < total; k += 32)
 	{
-		uint32_t lo = 0, hi = m.vertex_count;
-		while (hi - lo > 1)
-		{
-			uint32_t mid = (lo + hi) >> 1;
-			if (s_prefix[mid] <= k)
-				lo = mid;
-			else
-				hi = mid;
-		}
+		const uint32_t lo = scan::last_at_most(m.vertex_count, k, [&](uint32_t i) { return s_prefix[i]; });
 		uint32_t tri = data[offsets[s_mv[lo]] + (k - s_prefix[lo])];
 		uint32_t a = indices[tri * 3 + 0], b = indices[tri * 3 + 1], c = indices[tri * 3 + 2];
 		uint32_t extra = (used[a] < 0) + (used[b] < 0) + (used[c] < 0);
@@ -2564,7 +2547,7 @@ __global__ void __launch_bounds__(kCookWarps * 32) cook_build_kernel(const CookA
 	{
 		uint32_t v = base + lane;
 		uint32_t c = v < vertex_count ? counts[v] : 0u;
-		uint32_t incl = cook_warp_inclusive(c, lane);
+		uint32_t incl = scan::warp_inclusive(c, lane);
 		if (v < vertex_count)
 			offsets[v] = carry + incl - c;
 		carry += __shfl_sync(full, incl, 31);
@@ -2765,21 +2748,6 @@ __global__ void __launch_bounds__(kCookWarps * 32) cook_build_kernel(const CookA
 	}
 }
 
-// the job whose slots hold slot s: the last job starting at or before it
-__device__ __forceinline__ uint32_t cook_job_of_slot(const CookArgs& a, uint32_t s)
-{
-	uint32_t lo = 0, hi = a.job_count;
-	while (hi - lo > 1)
-	{
-		uint32_t mid = (lo + hi) >> 1;
-		if (a.jobs[mid].slot <= s)
-			lo = mid;
-		else
-			hi = mid;
-	}
-	return lo;
-}
-
 // One thread per meshlet: meshopt_optimizeMeshletLevel(level 1), then what appendMeshlet (scene.cpp:26-47) derives from
 // the meshlet's vertices: minVertex, shortRefs and the words it takes.
 __global__ void __launch_bounds__(128) cook_optimize_kernel(const CookArgs a)
@@ -2787,7 +2755,7 @@ __global__ void __launch_bounds__(128) cook_optimize_kernel(const CookArgs a)
 	uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
 	if (s >= a.slot_count)
 		return;
-	uint32_t j = cook_job_of_slot(a, s);
+	uint32_t j = scan::last_at_most(a.job_count, s, [&](uint32_t i) { return a.jobs[i].slot; });
 	const cook::CookJob& job = a.jobs[j];
 	if (s - job.slot >= a.job_meshlets[j])
 	{
@@ -2808,62 +2776,26 @@ __global__ void __launch_bounds__(128) cook_optimize_kernel(const CookArgs a)
 	a.slot_words[s] = (short_refs ? (r.z + 1u) / 2u : r.z) + (r.w * 3u + 3u) / 4u;
 }
 
-// exclusive scan of v over the block, returns the block total; s_warp holds 32 words
-__device__ __forceinline__ uint32_t cook_block_exclusive(uint32_t v, uint32_t& total, uint32_t* s_warp)
-{
-	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-	uint32_t incl = cook_warp_inclusive(v, lane);
-	if (lane == 31)
-		s_warp[warp] = incl;
-	__syncthreads();
-	uint32_t before = 0;
-	total = 0;
-	for (uint32_t w = 0; w < kCookScanThreads / 32; ++w)
-	{
-		before += w < warp ? s_warp[w] : 0u;
-		total += s_warp[w];
-	}
-	__syncthreads();
-	return before + incl - v;
-}
-
 // One block: LOD meshlet offsets (scene.cpp:274-275) and meshlet data offsets, both in job order; the totals and the
 // overflow flag.
 __global__ void __launch_bounds__(kCookScanThreads) cook_scan_kernel(const CookArgs a)
 {
-	__shared__ uint32_t s_warp[32];
-	uint64_t carry = 0;
-	for (uint32_t base = 0; base < a.job_count; base += kCookScanThreads)
-	{
-		uint32_t j = base + threadIdx.x;
-		uint32_t n = j < a.job_count ? a.job_meshlets[j] : 0u, total;
-		uint32_t before = cook_block_exclusive(n, total, s_warp);
-		if (j < a.job_count)
-		{
-			uint32_t first = uint32_t(carry + before);
-			a.job_first[j] = first;
-			NvcMeshLod& lod = a.meshes[a.jobs[j].mesh].lods[a.jobs[j].lod];
-			lod.meshletOffset = first;
-			lod.meshletCount = n;
-		}
-		carry += total;
-	}
-	uint64_t meshlets = carry;
-	carry = 0;
-	for (uint32_t base = 0; base < a.slot_count; base += kCookScanThreads)
-	{
-		uint32_t s = base + threadIdx.x;
-		uint32_t n = s < a.slot_count ? a.slot_words[s] : 0u, total;
-		uint32_t before = cook_block_exclusive(n, total, s_warp);
-		if (s < a.slot_count)
-			a.slot_data[s] = uint32_t(carry + before);
-		carry += total;
-	}
+	__shared__ uint32_t s_warp[kCookScanThreads / 32];
+	const uint64_t meshlets = scan::scan_tiles<kCookScanThreads>(
+	    a.job_count, uint64_t(0), s_warp, [&](uint32_t j) { return a.job_meshlets[j]; },
+	    [&](uint32_t j, uint64_t first) {
+		    a.job_first[j] = uint32_t(first);
+		    NvcMeshLod& lod = a.meshes[a.jobs[j].mesh].lods[a.jobs[j].lod];
+		    lod.meshletOffset = uint32_t(first);
+		    lod.meshletCount = a.job_meshlets[j];
+	    });
+	const uint64_t words = scan::scan_tiles<kCookScanThreads>(
+	    a.slot_count, uint64_t(0), s_warp, [&](uint32_t s) { return a.slot_words[s]; }, [&](uint32_t s, uint64_t first) { a.slot_data[s] = uint32_t(first); });
 	if (threadIdx.x == 0)
 	{
 		a.totals4[0] = meshlets > 0xffffffffull ? 0xffffffffu : uint32_t(meshlets);
-		a.totals4[1] = carry > 0xffffffffull ? 0xffffffffu : uint32_t(carry);
-		a.totals4[3] = (meshlets > a.meshlet_capacity || carry > a.meshletdata_capacity) ? 1u : 0u;
+		a.totals4[1] = words > 0xffffffffull ? 0xffffffffu : uint32_t(words);
+		a.totals4[3] = (meshlets > a.meshlet_capacity || words > a.meshletdata_capacity) ? 1u : 0u;
 	}
 }
 
@@ -2874,7 +2806,7 @@ __global__ void __launch_bounds__(128) cook_pack_kernel(const CookArgs a)
 	uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
 	if (s >= a.slot_count || a.totals4[3])
 		return;
-	uint32_t j = cook_job_of_slot(a, s);
+	uint32_t j = scan::last_at_most(a.job_count, s, [&](uint32_t i) { return a.jobs[i].slot; });
 	const cook::CookJob& job = a.jobs[j];
 	uint32_t local = s - uint32_t(job.slot);
 	if (local >= a.job_meshlets[j])
@@ -2946,7 +2878,7 @@ __device__ void spatial_radix_pass(uint32_t lane, uint32_t* dst, const uint32_t*
 	uint32_t sum = 0;
 	for (uint32_t q = 0; q < 32; ++q)
 		sum += hist[lane * 32 + q];
-	uint32_t run = cook_warp_inclusive(sum, lane) - sum;
+	uint32_t run = scan::warp_inclusive(sum, lane) - sum;
 	for (uint32_t q = 0; q < 32; ++q)
 	{
 		uint32_t c = hist[lane * 32 + q];
@@ -3265,7 +3197,7 @@ __global__ void __launch_bounds__(kSpatialWarps * 32) cook_spatial_kernel(const 
 	uint32_t marks = 0;
 	for (uint32_t i = lane; i < n; i += 32)
 		marks += boundary[i];
-	const uint32_t meshlet_count = __shfl_sync(full, cook_warp_inclusive(marks, lane), 31);
+	const uint32_t meshlet_count = __shfl_sync(full, scan::warp_inclusive(marks, lane), 31);
 	if (lane == 0)
 	{
 		const uint64_t meshlet_bound = cook::spatial_meshlets_bound(index_count);
@@ -3308,23 +3240,13 @@ __global__ void __launch_bounds__(kSpatialWarps * 32) cook_spatial_kernel(const 
 // then meshlet order); totals8[4] and the overflow flag.  Runs after cook_scan_kernel, before the pack kernels.
 __global__ void __launch_bounds__(kCookScanThreads) cook_vtx0_scan_kernel(const CookClrtArgs c)
 {
-	__shared__ uint32_t s_warp[32];
+	__shared__ uint32_t s_warp[kCookScanThreads / 32];
 	const CookArgs& a = c.base;
-	uint64_t carry = 0;
-	for (uint32_t base = 0; base < a.slot_count; base += kCookScanThreads)
-	{
-		uint32_t s = base + threadIdx.x, n = 0, total;
-		if (s < a.slot_count)
-		{
-			uint32_t j = cook_job_of_slot(a, s);
-			if (c.job_rt[j] && s - uint32_t(a.jobs[j].slot) < a.job_meshlets[j])
-				n = 4u * a.ml_records[s].z;
-		}
-		uint32_t before = cook_block_exclusive(n, total, s_warp);
-		if (s < a.slot_count)
-			c.slot_vtx0[s] = uint32_t(carry + before);
-		carry += total;
-	}
+	auto elements = [&](uint32_t s) {
+		const uint32_t j = scan::last_at_most(a.job_count, s, [&](uint32_t i) { return a.jobs[i].slot; });
+		return c.job_rt[j] && s - uint32_t(a.jobs[j].slot) < a.job_meshlets[j] ? 4u * a.ml_records[s].z : 0u;
+	};
+	const uint64_t carry = scan::scan_tiles<kCookScanThreads>(a.slot_count, uint64_t(0), s_warp, elements, [&](uint32_t s, uint64_t first) { c.slot_vtx0[s] = uint32_t(first); });
 	if (threadIdx.x == 0)
 	{
 		a.totals4[4] = carry > 0xffffffffull ? 0xffffffffu : uint32_t(carry);
@@ -3341,7 +3263,7 @@ __global__ void __launch_bounds__(128) cook_vtx0_pack_kernel(const CookClrtArgs 
 	uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
 	if (s >= a.slot_count || a.totals4[3])
 		return;
-	uint32_t j = cook_job_of_slot(a, s);
+	uint32_t j = scan::last_at_most(a.job_count, s, [&](uint32_t i) { return a.jobs[i].slot; });
 	const cook::CookJob& job = a.jobs[j];
 	if (!c.job_rt[j] || s - uint32_t(job.slot) >= a.job_meshlets[j])
 		return;
@@ -3457,20 +3379,23 @@ cudaError_t launch_cook_mesh_lods(const LodArgs& a, cudaStream_t stream)
 	return cudaGetLastError();
 }
 
-// ---- nvc_cook_mesh_vertices: appendMesh's vertex processing (nvc_vertices.cuh) ---------------------------------------------
-// exclusive scan of a.flags[0, n) into a.rank: block sums, their scan (one CTA), each block from its offset
-static void verts_scan(const VertexArgs& a, uint64_t n, cudaStream_t stream)
+// ---- the device-wide scan (nvc_scan.cuh) ----------------------------------------------------------------------------------
+// The exclusive scans of `rows` rows of n values each: row r of `out` is n + 1 long and ends with the row's total.
+// block_sums and block_offsets hold rows x ceil(n / scan::kScanItems) and rows x (that + 1) words.
+template <typename In, typename Out>
+static cudaError_t launch_scan(const In* in, uint64_t n, uint32_t rows, uint32_t* block_sums, unsigned long long* block_offsets, Out* out, cudaStream_t stream)
 {
-	using namespace verts;
-	const uint32_t blocks = uint32_t((n + verts::kScanItems - 1) / verts::kScanItems);
-	if (blocks)
-		verts_scan_reduce_kernel<<<blocks, verts::kThreads, 0, stream>>>(a.flags, n, a.block_sums);
-	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
-	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_sums, blocks, a.offsets);
-	if (blocks)
-		verts_scan_apply_kernel<<<blocks, verts::kThreads, 0, stream>>>(a.flags, n, a.offsets, a.rank);
+	using namespace scan;
+	if (n == 0)
+		return cudaMemsetAsync(out, 0, rows * sizeof(Out), stream); // the totals
+	const uint32_t blocks = uint32_t((n + scan::kScanItems - 1) / scan::kScanItems);
+	reduce_kernel<In><<<dim3(blocks, rows), scan::kThreads, 0, stream>>>(in, n, block_sums);
+	offsets_kernel<<<rows, scan::kOffsetsThreads, 0, stream>>>(block_sums, blocks, block_offsets);
+	apply_kernel<In, Out><<<dim3(blocks, rows), scan::kThreads, 0, stream>>>(in, n, block_offsets, out);
+	return cudaSuccess;
 }
 
+// ---- nvc_cook_mesh_vertices: appendMesh's vertex processing (nvc_vertices.cuh) ---------------------------------------------
 uint64_t vertex_cache_words(uint32_t vertices, uint32_t indices)
 {
 	return verts::carve(vertices, indices, nullptr, nullptr);
@@ -3485,6 +3410,10 @@ cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream)
 	auto fill = [&](void* p, int value, size_t bytes) {
 		if (e == cudaSuccess && bytes)
 			e = cudaMemsetAsync(p, value, bytes, stream);
+	};
+	auto scan_flags = [&](uint32_t n) {
+		if (e == cudaSuccess)
+			e = launch_scan(a.flags, n, 1, a.block_sums, a.offsets, a.rank, stream);
 	};
 	fill(a.totals4, 0, 16);
 	fill(a.rejected, 0, M);
@@ -3502,7 +3431,7 @@ cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream)
 		verts_filter_insert_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
 		verts_filter_flag_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
 	}
-	verts_scan(a, T, stream);
+	scan_flags(T);
 	if (T)
 		verts_filter_compact_kernel<<<grid(T), verts::kThreads, 0, stream>>>(a);
 	if (M)
@@ -3516,7 +3445,7 @@ cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream)
 		verts_class_insert_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
 		verts_class_flag_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
 	}
-	verts_scan(a, N, stream);
+	scan_flags(N);
 	if (M)
 		verts_mesh_kernel<<<grid(M), verts::kThreads, 0, stream>>>(a);
 	if (S)
@@ -3534,7 +3463,7 @@ cudaError_t launch_cook_mesh_vertices(const VertexArgs& a, cudaStream_t stream)
 		verts_fetch_first_kernel<<<grid(N), verts::kThreads, 0, stream>>>(a);
 	if (S)
 		verts_fetch_flag_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
-	verts_scan(a, N, stream);
+	scan_flags(N);
 	if (S)
 		verts_fetch_scatter_kernel<<<grid(S), verts::kThreads, 0, stream>>>(a);
 	if (N)
@@ -3553,8 +3482,8 @@ cudaError_t launch_obj_lines(const ObjArgs& a, cudaStream_t stream)
 	using namespace obj;
 	if (a.tile_count)
 		obj_tile_count_kernel<<<a.tile_count, obj::kThreads, 0, stream>>>(a);
-	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
-	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.tile_lines, a.tile_count, a.tile_offsets);
+	void (*offsets)(const uint32_t*, uint32_t, unsigned long long*) = scan::offsets_kernel;
+	offsets<<<1, scan::kOffsetsThreads, 0, stream>>>(a.tile_lines, a.tile_count, a.tile_offsets);
 	return cudaGetLastError();
 }
 
@@ -3571,11 +3500,9 @@ cudaError_t launch_obj_count(const ObjArgs& a, cudaStream_t stream)
 	}
 	obj_file_kernel<<<obj_grid(a.file_count), obj::kThreads, 0, stream>>>(a);
 	obj_classify_kernel<<<obj_grid(a.line_slots), obj::kThreads, 0, stream>>>(a);
-	obj_scan_reduce_kernel<<<dim3(a.scan_blocks, kFields), obj::kThreads, 0, stream>>>(a);
-	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
-	for (uint32_t k = 0; k < kFields; ++k)
-		scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_sums + size_t(k) * a.scan_blocks, a.scan_blocks, a.block_offsets + size_t(k) * (a.scan_blocks + 1));
-	obj_scan_apply_kernel<<<dim3(a.scan_blocks, kFields), obj::kThreads, 0, stream>>>(a);
+	e = launch_scan(a.counts, a.line_slots, kFields, a.block_sums, a.block_offsets, a.prefix, stream);
+	if (e != cudaSuccess)
+		return e;
 	obj_info_kernel<<<obj_grid(a.file_count), obj::kThreads, 0, stream>>>(a);
 	return cudaGetLastError();
 }
@@ -3945,11 +3872,11 @@ cudaError_t launch_encode_vertices(const VertexEncodeArgs& a, uint32_t stride, c
 	void (*estimate)(VertexEncodeArgs) = stride == 16 ? cache::encode_vertex_estimate_kernel<16> : cache::encode_vertex_estimate_kernel<8>;
 	void (*measure)(VertexEncodeArgs) = stride == 16 ? cache::encode_vertex_blocks_kernel<16, false> : cache::encode_vertex_blocks_kernel<8, false>;
 	void (*write)(VertexEncodeArgs) = stride == 16 ? cache::encode_vertex_blocks_kernel<16, true> : cache::encode_vertex_blocks_kernel<8, true>;
-	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	void (*offsets)(const uint32_t*, uint32_t, unsigned long long*) = scan::offsets_kernel;
 	if (a.vertex_count > 1) // one vertex keeps channel 0 everywhere
 		estimate<<<estimate_blocks, cache::kEstimateThreads, 0, stream>>>(a);
 	measure<<<grid, cache::kEncodeWarps * 32, 0, stream>>>(a);
-	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_bytes, a.blocks, a.offsets);
+	offsets<<<1, scan::kOffsetsThreads, 0, stream>>>(a.block_bytes, a.blocks, a.offsets);
 	write<<<grid, cache::kEncodeWarps * 32, 0, stream>>>(a);
 	return cudaGetLastError();
 }
@@ -3962,10 +3889,10 @@ cudaError_t launch_encode_meshlets(const MeshletEncodeArgs& a, cudaStream_t stre
 	const uint32_t grid = (a.meshlet_count + cache::kMeshletEncodeThreads - 1) / cache::kMeshletEncodeThreads;
 	void (*measure)(MeshletEncodeArgs) = cache::encode_meshlets_kernel<false>;
 	void (*write)(MeshletEncodeArgs) = cache::encode_meshlets_kernel<true>;
-	void (*scan)(const uint32_t*, uint32_t, unsigned long long*) = cache::encode_scan_kernel;
+	void (*offsets)(const uint32_t*, uint32_t, unsigned long long*) = scan::offsets_kernel;
 	if (a.meshlet_count)
 		measure<<<grid, cache::kMeshletEncodeThreads, 0, stream>>>(a);
-	scan<<<1, cache::kEncodeScanThreads, 0, stream>>>(a.block_bytes, a.meshlet_count, a.offsets);
+	offsets<<<1, scan::kOffsetsThreads, 0, stream>>>(a.block_bytes, a.meshlet_count, a.offsets);
 	if (a.meshlet_count)
 		write<<<grid, cache::kMeshletEncodeThreads, 0, stream>>>(a);
 	return cudaGetLastError();

@@ -3,12 +3,12 @@
 //
 // Each line is a pure function of its bytes and of the v / vt / vn lines before it in its file; the only other link between
 // lines is the reader's 64 KiB rule.  So the parse is data-parallel over lines, in four launch groups:
-//   lines   per 4 KiB tile (256 threads x 16 bytes) its '\n' count, then their scan (nvc_cache_encode.cuh's encode_scan_kernel).
+//   lines   per 4 KiB tile (256 threads x 16 bytes) its '\n' count, then their scan (nvc_scan.cuh's offsets_kernel).
 //   count   each '\n' is written to its line slot; a full 64 KiB block without '\n' is flagged and the smallest flag of a file
 //           is where the reader stops; one thread per line classifies it from its first bytes (a face line is walked to count
-//           its records) and writes its counts (obj::Field), which are scanned as the vertex cooker scans its flags: per-block
-//           sums, encode_scan_kernel over them, each block from its offset.  The scans run over all files at once: a file's
-//           values are the prefix at its line minus the prefix at its first line.
+//           its records) and writes its counts (obj::Field), one row per field, which nvc_scan.cuh's device-wide scan
+//           turns into prefixes, all rows in the same launches.  The scans run over all files at once: a file's values are
+//           the prefix at its line minus the prefix at its first line.
 //   parse   one thread per line writes its numbers, its index records and its face (window start, size, first corner); then
 //           one thread per face checks the window loadObj reads (the running sum of face sizes, so orphan records shift it)
 //           against the file's final counts.
@@ -20,8 +20,9 @@
 // negative, so the float is 0xffc00000 whatever the device's NaN bits.  Indices: parse_int in 32-bit wrapping arithmetic.
 #pragma once
 
-#include "nvc_cache_encode.cuh"
 #include "nvc_cook.cuh"
+#include "nvc_internal.h"
+#include "nvc_scan.cuh"
 
 namespace nvc
 {
@@ -29,7 +30,6 @@ namespace obj
 {
 
 constexpr uint32_t kThreads = 256;
-constexpr uint32_t kScanPerThread = kScanItems / kThreads;
 constexpr uint32_t kNaN = 0xffc00000u;
 
 // ---- one line's bytes -----------------------------------------------------------------------------------------------------
@@ -209,25 +209,9 @@ __device__ __forceinline__ uint32_t classify(const Line& l, uint32_t start, uint
 	return kOther;
 }
 
-// the last i in [0, n) with key(i) <= x (key non-decreasing, key(0) <= x)
-template <typename Key>
-__device__ __forceinline__ uint32_t last_at_most(uint32_t n, uint64_t x, const Key& key)
-{
-	uint32_t lo = 0, hi = n;
-	while (hi - lo > 1)
-	{
-		const uint32_t mid = (lo + hi) / 2;
-		if (key(mid) <= x)
-			lo = mid;
-		else
-			hi = mid;
-	}
-	return lo;
-}
-
 __device__ __forceinline__ uint32_t file_of_slot(const ObjArgs& a, uint32_t s)
 {
-	return last_at_most(a.file_count, s, [&](uint32_t f) { return uint64_t(a.state[f].first_line); });
+	return scan::last_at_most(a.file_count, s, [&](uint32_t f) { return a.state[f].first_line; });
 }
 
 __device__ __forceinline__ Line line_of(const ObjArgs& a, uint32_t f, uint32_t s, uint32_t& start)
@@ -255,7 +239,7 @@ struct TileBytes
 __device__ __forceinline__ TileBytes tile_bytes(const ObjArgs& a, uint32_t t)
 {
 	TileBytes r;
-	r.file = last_at_most(a.file_count, t, [&](uint32_t f) { return uint64_t(a.files[f].tile_base); });
+	r.file = scan::last_at_most(a.file_count, t, [&](uint32_t f) { return a.files[f].tile_base; });
 	const File& f = a.files[r.file];
 	r.pos = (t - f.tile_base) * kTileBytes + threadIdx.x * 16u;
 	r.n = r.pos < f.size ? min(16u, f.size - r.pos) : 0u;
@@ -282,20 +266,9 @@ __device__ __forceinline__ uint32_t newlines(const TileBytes& r)
 __global__ void __launch_bounds__(kThreads) obj_tile_count_kernel(const ObjArgs a)
 {
 	__shared__ uint32_t s_warp[kThreads / 32];
-	const TileBytes r = tile_bytes(a, blockIdx.x);
-	uint32_t c = newlines(r);
-	for (uint32_t d = 16; d > 0; d >>= 1)
-		c += __shfl_down_sync(0xffffffffu, c, d);
-	if ((threadIdx.x & 31u) == 0)
-		s_warp[threadIdx.x >> 5] = c;
-	__syncthreads();
+	const uint32_t total = scan::block_sum<kThreads>(newlines(tile_bytes(a, blockIdx.x)), s_warp);
 	if (threadIdx.x == 0)
-	{
-		uint32_t total = 0;
-		for (uint32_t w = 0; w < kThreads / 32; ++w)
-			total += s_warp[w];
 		a.tile_lines[blockIdx.x] = total;
-	}
 }
 
 // ---- count ----------------------------------------------------------------------------------------------------------------
@@ -304,22 +277,9 @@ __global__ void __launch_bounds__(kThreads) obj_tile_count_kernel(const ObjArgs 
 __global__ void __launch_bounds__(kThreads) obj_line_end_kernel(const ObjArgs a)
 {
 	__shared__ uint32_t s_warp[kThreads / 32];
-	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
 	const TileBytes r = tile_bytes(a, blockIdx.x);
-	const uint32_t c = newlines(r);
-	uint32_t x = c;
-	for (uint32_t d = 1; d < 32; d <<= 1)
-	{
-		const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
-		if (lane >= d)
-			x += y;
-	}
-	if (lane == 31)
-		s_warp[warp] = x;
-	__syncthreads();
-	uint64_t slot = a.tile_offsets[blockIdx.x] + r.file + x - c;
-	for (uint32_t w = 0; w < warp; ++w)
-		slot += s_warp[w];
+	uint32_t total;
+	uint64_t slot = a.tile_offsets[blockIdx.x] + r.file + scan::block_exclusive<kThreads>(newlines(r), s_warp, total);
 	for (uint32_t k = 0; k < 16; ++k)
 		if (k < r.n && r.b[k] == '\n')
 			a.line_end[slot++] = r.pos + k;
@@ -331,7 +291,7 @@ __global__ void __launch_bounds__(kThreads) obj_cut_kernel(const ObjArgs a)
 	const uint32_t t = blockIdx.x * kThreads + threadIdx.x;
 	if (t >= a.tile_count)
 		return;
-	const uint32_t f = last_at_most(a.file_count, t, [&](uint32_t g) { return uint64_t(a.files[g].tile_base); });
+	const uint32_t f = scan::last_at_most(a.file_count, t, [&](uint32_t g) { return a.files[g].tile_base; });
 	const uint32_t j = t - a.files[f].tile_base;
 	if (j % kTilesPerBlock != 0 || uint64_t(j + kTilesPerBlock) * kTileBytes > a.files[f].size)
 		return;
@@ -392,69 +352,6 @@ __global__ void __launch_bounds__(kThreads) obj_classify_kernel(const ObjArgs a)
 	}
 	for (uint32_t k = 0; k < kFields; ++k)
 		a.counts[k * L + s] = c[k];
-}
-
-// per-block sums of field blockIdx.y
-__global__ void __launch_bounds__(kThreads) obj_scan_reduce_kernel(const ObjArgs a)
-{
-	__shared__ uint32_t s_warp[kThreads / 32];
-	const uint64_t L = a.line_slots;
-	const uint32_t* counts = a.counts + blockIdx.y * L;
-	const uint64_t first = uint64_t(blockIdx.x) * kScanItems + uint64_t(threadIdx.x) * kScanPerThread;
-	uint32_t sum = 0;
-	for (uint32_t k = 0; k < kScanPerThread; ++k)
-		sum += first + k < L ? counts[first + k] : 0u;
-	for (uint32_t d = 16; d > 0; d >>= 1)
-		sum += __shfl_down_sync(0xffffffffu, sum, d);
-	if ((threadIdx.x & 31u) == 0)
-		s_warp[threadIdx.x >> 5] = sum;
-	__syncthreads();
-	if (threadIdx.x == 0)
-	{
-		uint32_t total = 0;
-		for (uint32_t w = 0; w < kThreads / 32; ++w)
-			total += s_warp[w];
-		a.block_sums[blockIdx.y * a.scan_blocks + blockIdx.x] = total;
-	}
-}
-
-// prefix[field][i] = block offset + the counts before i in its block; the total at L
-__global__ void __launch_bounds__(kThreads) obj_scan_apply_kernel(const ObjArgs a)
-{
-	__shared__ uint32_t s_warp[kThreads / 32];
-	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-	const uint64_t L = a.line_slots;
-	const uint32_t* counts = a.counts + blockIdx.y * L;
-	const unsigned long long* offsets = a.block_offsets + blockIdx.y * (uint64_t(a.scan_blocks) + 1);
-	unsigned long long* out = a.prefix + blockIdx.y * (L + 1);
-	const uint64_t first = uint64_t(blockIdx.x) * kScanItems + uint64_t(threadIdx.x) * kScanPerThread;
-	uint32_t v[kScanPerThread], sum = 0;
-	for (uint32_t k = 0; k < kScanPerThread; ++k)
-	{
-		v[k] = first + k < L ? counts[first + k] : 0u;
-		sum += v[k];
-	}
-	uint32_t x = sum;
-	for (uint32_t d = 1; d < 32; d <<= 1)
-	{
-		const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
-		if (lane >= d)
-			x += y;
-	}
-	if (lane == 31)
-		s_warp[warp] = x;
-	__syncthreads();
-	unsigned long long before = offsets[blockIdx.x] + (x - sum);
-	for (uint32_t w = 0; w < warp; ++w)
-		before += s_warp[w];
-	for (uint32_t k = 0; k < kScanPerThread; ++k)
-		if (first + k < L)
-		{
-			out[first + k] = before;
-			before += v[k];
-		}
-	if (blockIdx.x == 0 && threadIdx.x == 0)
-		out[L] = offsets[a.scan_blocks];
 }
 
 // one thread per file: its final counts, its arrays' bases, its info
@@ -577,7 +474,7 @@ __global__ void __launch_bounds__(kThreads) obj_expand_kernel(const ObjArgs a)
 	const uint64_t c = uint64_t(blockIdx.x) * kThreads + threadIdx.x;
 	if (c >= a.corner_count)
 		return;
-	const uint32_t i = last_at_most(a.face_count, c, [&](uint32_t k) { return uint64_t(a.faces[k].corner); });
+	const uint32_t i = scan::last_at_most(a.face_count, c, [&](uint32_t k) { return a.faces[k].corner; });
 	const Face face = a.faces[i];
 	const uint32_t j = uint32_t(c - face.corner), r = j % 3;
 	const uint32_t fan = r == 0 ? 0 : j / 3 + r; // (c0, c(k+1), c(k+2)) for triangle k

@@ -19,11 +19,12 @@
 //           second table, which keeps the smallest `first` of its members; each class flags that position, and the scan
 //           of the flags ranks the classes in the order of their first reference, which is generateVertexRemap's order.
 //   fetch   first use of each vertex over the optimised indices by atomicMin, flags, scan, as above.
-// A scan is three launches: per-block sums of kScanItems flags, nvc_cache_encode.cuh's encode_scan_kernel over the sums,
-// then each block scans its flags from its offset.  Nothing spins, so the kernels run as they are under the SIMT emulation too.
+// A scan is nvc_scan.cuh's device-wide scan of the flags into `rank`, the total at rank[n].  Nothing spins, so the kernels
+// run as they are under the SIMT emulation too.
 #pragma once
 
 #include "nvc_lods.cuh"
+#include "nvc_scan.cuh"
 
 namespace nvc
 {
@@ -32,7 +33,6 @@ namespace verts
 
 constexpr uint32_t kNone = ~0u;
 constexpr uint32_t kThreads = 256;
-constexpr uint32_t kScanPerThread = kScanItems / kThreads;
 
 // the vertex cache optimiser's arrays of a mesh with at most V vertices and N indices (lods::carve's layout for them);
 // returns the mesh's words.  base == nullptr: size only
@@ -77,35 +77,20 @@ __device__ __forceinline__ uint32_t hash_mix(uint64_t h, uint64_t k)
 	return uint32_t(h >> 32) ^ uint32_t(h);
 }
 
-// the largest i < n with base(i) <= x: the mesh whose range holds x (an empty mesh shares its base with the next one)
-template <typename F>
-__device__ __forceinline__ uint32_t find_mesh(uint32_t n, uint32_t x, const F& base)
-{
-	uint32_t lo = 0, hi = n;
-	while (hi - lo > 1)
-	{
-		const uint32_t mid = (lo + hi) >> 1;
-		if (base(mid) <= x)
-			lo = mid;
-		else
-			hi = mid;
-	}
-	return lo;
-}
-
+// the mesh whose range holds a triangle, slot or position (an empty mesh shares its base with the next one)
 __device__ __forceinline__ uint32_t job_of_triangle(const VertexArgs& a, uint32_t t)
 {
-	return find_mesh(a.mesh_count, t, [&](uint32_t m) { return a.jobs[m].tri_base; });
+	return scan::last_at_most(a.mesh_count, t, [&](uint32_t m) { return a.jobs[m].tri_base; });
 }
 
 __device__ __forceinline__ uint32_t job_of_slot(const VertexArgs& a, uint32_t s)
 {
-	return find_mesh(a.mesh_count, s, [&](uint32_t m) { return a.jobs[m].slot_base; });
+	return scan::last_at_most(a.mesh_count, s, [&](uint32_t m) { return a.jobs[m].slot_base; });
 }
 
 __device__ __forceinline__ uint32_t job_of_position(const VertexArgs& a, uint32_t p)
 {
-	return find_mesh(a.mesh_count, p, [&](uint32_t m) { return a.index_base[m]; });
+	return scan::last_at_most(a.mesh_count, p, [&](uint32_t m) { return a.index_base[m]; });
 }
 
 __device__ __forceinline__ uint64_t position_key(const NvcVertex& v)
@@ -126,70 +111,6 @@ __device__ __forceinline__ bool triangle_key(const VertexArgs& a, const VertexJo
 	k[1] = y_least ? z : z_least ? x : y;
 	k[2] = y_least ? x : z_least ? y : z;
 	return true;
-}
-
-// ---- scans: exclusive scan of n byte flags into 32-bit ranks (the count of any flags fits: n < 2^32) --------------------
-
-// per block of kScanItems flags: their sum
-__global__ void __launch_bounds__(kThreads) verts_scan_reduce_kernel(const uint8_t* flags, uint64_t n, uint32_t* block_sums)
-{
-	__shared__ uint32_t s_warp[kThreads / 32];
-	const uint64_t first = uint64_t(blockIdx.x) * kScanItems + uint64_t(threadIdx.x) * kScanPerThread;
-	uint32_t sum = 0;
-	for (uint32_t k = 0; k < kScanPerThread; ++k)
-		sum += first + k < n ? flags[first + k] : 0u;
-	for (uint32_t d = 16; d > 0; d >>= 1)
-		sum += __shfl_down_sync(0xffffffffu, sum, d);
-	if ((threadIdx.x & 31u) == 0)
-		s_warp[threadIdx.x >> 5] = sum;
-	__syncthreads();
-	if (threadIdx.x == 0)
-	{
-		uint32_t total = 0;
-		for (uint32_t w = 0; w < kThreads / 32; ++w)
-			total += s_warp[w];
-		block_sums[blockIdx.x] = total;
-	}
-}
-
-// rank[i] = offsets[block] + the flags before i in its block
-__global__ void __launch_bounds__(kThreads) verts_scan_apply_kernel(const uint8_t* flags, uint64_t n, const unsigned long long* offsets, uint32_t* rank)
-{
-	__shared__ uint32_t s_warp[kThreads / 32];
-	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-	const uint64_t first = uint64_t(blockIdx.x) * kScanItems + uint64_t(threadIdx.x) * kScanPerThread;
-	uint8_t f[kScanPerThread];
-	uint32_t v = 0;
-	for (uint32_t k = 0; k < kScanPerThread; ++k)
-	{
-		f[k] = first + k < n ? flags[first + k] : 0;
-		v += f[k];
-	}
-	uint32_t x = v;
-	for (uint32_t d = 1; d < 32; d <<= 1)
-	{
-		const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
-		if (lane >= d)
-			x += y;
-	}
-	if (lane == 31)
-		s_warp[warp] = x;
-	__syncthreads();
-	uint32_t before = uint32_t(offsets[blockIdx.x]) + x - v;
-	for (uint32_t w = 0; w < warp; ++w)
-		before += s_warp[w];
-	for (uint32_t k = 0; k < kScanPerThread; ++k)
-		if (first + k < n)
-		{
-			rank[first + k] = before;
-			before += f[k];
-		}
-}
-
-// the last scan (of n flags) at i <= n: rank[i], or the total at n
-__device__ __forceinline__ uint32_t scan_at(const VertexArgs& a, uint64_t i, uint64_t n)
-{
-	return i < n ? a.rank[i] : uint32_t(a.offsets[(n + kScanItems - 1) / kScanItems]);
 }
 
 // ---- rejection and the filter ----------------------------------------------------------------------------------------------
@@ -273,9 +194,9 @@ __global__ void __launch_bounds__(kThreads) verts_index_base_kernel(const Vertex
 	const uint32_t m = blockIdx.x * kThreads + threadIdx.x;
 	if (m >= a.mesh_count)
 		return;
-	a.index_base[m] = 3 * scan_at(a, a.jobs[m].tri_base, a.tri_count);
+	a.index_base[m] = 3 * a.rank[a.jobs[m].tri_base];
 	if (m == 0)
-		a.totals4[1] = 3 * scan_at(a, a.tri_count, a.tri_count);
+		a.totals4[1] = 3 * a.rank[a.tri_count];
 	if (a.rejected[m])
 		atomicAdd(&a.totals4[2], 1u);
 }
@@ -360,10 +281,10 @@ __global__ void __launch_bounds__(kThreads) verts_mesh_kernel(const VertexArgs a
 		return;
 	const uint32_t n = a.totals4[1];
 	const uint32_t ib = a.index_base[m], ie = m + 1 < a.mesh_count ? a.index_base[m + 1] : n;
-	const uint32_t vb = scan_at(a, ib, a.position_count), ve = scan_at(a, ie, a.position_count);
+	const uint32_t vb = a.rank[ib], ve = a.rank[ie];
 	a.vertex_base[m] = vb;
 	if (m == 0)
-		a.totals4[0] = scan_at(a, n, a.position_count);
+		a.totals4[0] = a.rank[n];
 	NvcMesh mesh = {};
 	mesh.vertexOffset = vb;
 	mesh.vertexCount = ve - vb;
